@@ -2,7 +2,7 @@
 """Benchmark of the DDPM sampling hot path (BASELINE.json metric: mel-frames/sec,
 base_with_context, 1000-step DDPM).
 
-  python bench.py --gpus N --steps K --warmup W        # this repo's sm_100a path
+  python bench.py --gpus N --steps K --warmup W        # this repo's sm_90a path
   python bench.py --impl reference ...                 # the CPU oracle port on the host cores
 
 A "step" is one pass of the hot path over one batch: `predict` of `--segments` independent
@@ -281,7 +281,7 @@ def workload_config(args, t5, lengths, segments):
       'segments_per_gpu': segments, 'diffusion_steps': args.diffusion_steps,
       'emb_dim': t5.emb_dim, 'layers': t5.num_decoder_layers,
       'l2_policy': 'working set per diffusion step (weights 227 MB + cross K/V 85 MB/segment) '
-                   'exceeds the 126 MB L2; no explicit flush needed',
+                   'exceeds the 50 MB L2; no explicit flush needed',
       'parallelism': f'dp{args.gpus} (independent segments, no collective in the loop)',
   }
 
@@ -291,8 +291,8 @@ def peaks():
   if os.path.exists(p):
     with open(p) as f:
       j = json.load(f)
-    return j.get('bf16_tflops_sustained', 1388.2), j.get('hbm_gbs', 6483.9), 'measured'
-  return 1400.0, 6650.0, 'fallback'
+    return j.get('bf16_tflops_sustained', 989.0), j.get('hbm_gbs', 3350.0), 'measured'
+  return 989.0, 3350.0, 'H100 SXM data sheet (dense bf16, HBM3; a 700 W card)'
 
 
 KERNEL_CLASS_KEYS = ('gemm', 'attention_combine', 'attention', 'rmsnorm', 'sampler')
@@ -359,7 +359,7 @@ def graph_timeline(eng, seed=2):
 
 
 def measure_gemm_traffic(args, timeout_s=240):
-  """dram__bytes_read + write of the dominant kernel (CTA-pair GEMM), per launch, from an ncu pass
+  """dram__bytes_read + write of the dominant kernel (bf16 GEMM), per launch, from an ncu pass
   over one uncaptured diffusion step of this very workload (tools/profile_step.py in a child
   process; two metrics = one replay pass).  Returns a dict, or {'unavailable': why}."""
   import shutil
@@ -375,7 +375,7 @@ def measure_gemm_traffic(args, timeout_s=240):
   if skip is None or args.precision != 'bf16':
     return {'unavailable': 'launch indices are tabulated for the base bf16 workload only'}
   cmd = [ncu, '--metrics', 'dram__bytes_read.sum,dram__bytes_write.sum', '--clock-control', 'none',
-         '-k', 'regex:gemm_bf16_tcgen05_pair', '-s', str(skip), '-c', '74', '--csv', '--log-file', log,
+         '-k', 'regex:gemm_bf16_wgmma', '-s', str(skip), '-c', '74', '--csv', '--log-file', log,
          sys.executable, os.path.join(ROOT, 'tools', 'profile_step.py'), '--model', args.model,
          '--segments', str(args.segments), '--diffusion-steps', str(args.diffusion_steps)]
   try:
@@ -403,7 +403,7 @@ def measure_gemm_traffic(args, timeout_s=240):
     return {'unavailable': f'no dram__bytes rows in the ncu log (rc {r.returncode}): '
                            f'{(r.stderr or r.stdout)[-200:]}'}
   return {'dram_bytes_per_launch': total / len(ids), 'launches': len(ids),
-          'how': 'ncu dram__bytes_read.sum + dram__bytes_write.sum over the 74 CTA-pair GEMM '
+          'how': 'ncu dram__bytes_read.sum + dram__bytes_write.sum over the 74 GEMM '
                  'launches of one uncaptured diffusion step, measured in this run'}
 
 
@@ -538,6 +538,11 @@ def run_ours(args):
     return float(t.item()) / 1e3, wall, clocks, eng_mod.launch_count() - launches0
 
   sec, wall, clocks, launches = timed(device_step, args.warmup, args.steps)
+  if args.dump_outputs and rank == 0:
+    # what the last timed step returned to its caller (inputs and seed are fixed, so two builds
+    # of the library can be compared output for output)
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    np.save(os.path.join(args.dump_outputs, 'mel.npy'), d_mel.float().cpu().numpy())
   frames = world * B * lengths['targets'] * args.steps
   value = frames / sec
   sec_e2e, wall_e2e, clocks_e2e, _ = timed(host_step, max(1, args.warmup // 2), args.steps)
@@ -549,7 +554,7 @@ def run_ours(args):
     song_result = single_song_sample(t5, diff, lengths, local, segments=args.song_segments,
                                      world=world)
 
-  # ---- roofline of the dominant kernel class (tcgen05 GEMM), CUDA events per launch -------
+  # ---- roofline of the dominant kernel class (wgmma GEMM), CUDA events per launch -------
   prof = None
   if rank == 0:
     eng.encode(d_tok, d_ctx, d_msk)
@@ -575,18 +580,11 @@ def run_ours(args):
     if world == 1 and not args.no_traffic:
       traffic_info = measure_gemm_traffic(args)
       traffic = traffic_info.get('dram_bytes_per_launch')
-    if traffic is None:
-      tpath = os.path.join(ROOT, 'profiles', 'gemm_traffic.json')
-      if os.path.exists(tpath):
-        with open(tpath) as f:
-          traffic = json.load(f).get('dram_bytes_per_launch')
-        traffic_info = dict(traffic_info, fallback='profiles/gemm_traffic.json (recorded by an '
-                            'earlier ncu --set full capture, not measured in this run)')
     g_crit = (timeline or {}).get('critical_path_us_by_class', {}).get('gemm')
     roofline = {
-        'kernel': 'gemm_bf16_tcgen05_pair_kernel', 'bound': 'tensor',
+        'kernel': 'gemm_bf16_wgmma_kernel', 'bound': 'tensor',
         'achieved': gemm_tf, 'peak': peak_tf, 'unit': 'TFLOP/s',
-        'frac': gemm_tf / peak_tf, 'peak_source': f'{peak_kind} (bf16 sustained)',
+        'frac': gemm_tf / peak_tf, 'peak_source': f'{peak_kind}',
         'traffic': traffic, 'traffic_source': traffic_info,
         'algorithmic_bytes_per_launch': g['bytes'] / max(g['launches'], 1),
         # the same FLOPs over the time the class adds to the replayed step graph (PDL overlap)
@@ -672,10 +670,17 @@ def main():
   ap.add_argument('--no-cpu-baseline', action='store_true')
   ap.add_argument('--no-song', action='store_true',
                   help='skip the batch-1 chained-song sample (BASELINE config 5)')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='write what the last timed device step (engine encode + sample) returned to '
+                       'DIR/mel.npy (float32 [segments, frames, 128]); the host-batch (e2e) pass is '
+                       'not dumped; --impl ours only')
   ap.add_argument('--song-segments', type=int, default=12,
                   help='segments of the chained song (12 = 61.44 s, BASELINE config 5)')
   args = ap.parse_args()
   if args.impl == 'reference':
+    if args.dump_outputs:
+      ap.error('--dump-outputs applies to --impl ours (the reference arm extrapolates from a '
+               'bounded sample and computes no mel frames)')
     run_reference(args)
   else:
     run_ours(args)

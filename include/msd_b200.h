@@ -1,4 +1,4 @@
-/* msd_b200.h -- C ABI of libmsd_b200.so: the B200 (sm_100a) implementation of the DDPM
+/* msd_b200.h -- C ABI of libmsd_b200.so: the H100 (sm_90a) implementation of the DDPM
  * sampling hot path of magenta/music-spectrogram-diffusion.
  *
  * The reference has no FFI/plugin layer (it is pure Python on JAX/XLA); the drop-in boundary
@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define MSD_B200_ABI_VERSION 4
+#define MSD_B200_ABI_VERSION 5
 
 typedef struct msd_ctx msd_ctx;
 
@@ -169,8 +169,8 @@ uint64_t msd_launch_count(void);
 int msd_op_dense(const float* a, const float* w, int32_t M, int32_t N, int32_t K, float* out,
                  void* stream);
 
-/* Same, selecting the kernel: variant 0 = CTA-pair persistent kernel (default), 1 = single-CTA
- * kernel; block_n 0 = auto or one of 64/128/192/256 (192 only with variant 0). */
+/* Same, selecting the tile-width choice: variant 0 = widest tile that fills the SMs (default),
+ * 1 = power-of-two widths only; block_n 0 = auto or one of 64/128/192/256 (192 only with variant 0). */
 int msd_op_dense_variant(const float* a, const float* w, int32_t M, int32_t N, int32_t K,
                          float* out, int32_t variant, int32_t block_n, void* stream);
 
@@ -181,9 +181,9 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
                    int32_t block_n, int32_t iters, float* ms_out);
 
 /* Micro-benchmark hook: average milliseconds of `iters` back-to-back launches of the bf16
- * attention kernel (+ its combine kernel when the split is not merged in-kernel) on scratch
+ * attention kernel (+ its combine kernel when the keys are split) on scratch
  * buffers filled with small pseudo-random values; kv_static as in the decoder's cross-attention.
- * The instance / split is chosen as in production (or forced by MSD_ATTN_BKV / _SPLITS / _MERGE). */
+ * The instance / split is chosen as in production (or forced by MSD_ATTN_BKV / _SPLITS). */
 int msd_bench_attention(int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32_t iters,
                         float* ms_out);
 
@@ -192,12 +192,6 @@ int msd_bench_attention(int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32
  * out [nb, Lq, heads*64] f32 device. */
 int msd_op_attention(const float* q, const float* k, const float* v, const int32_t* key_mask,
                      int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, float* out, void* stream);
-
-/* Same with a debugging trace: `trace` (device, int64 [2][64][8], may be NULL) receives clock64
- * stamps of the softmax phases of CTA (0,0,0) for each key block (see attention_tcgen05.cu). */
-int msd_op_attention_trace(const float* q, const float* k, const float* v,
-                           const int32_t* key_mask, int32_t nb, int32_t heads, int32_t Lq,
-                           int32_t Lk, float* out, int64_t* trace, void* stream);
 
 /* DenseGeneral with each fused epilogue of the hot path (kernels.h GemmEpilogue), for unit parity:
  *   0 bf16 out                      out [M, N]            = bf16(a w)

@@ -1,1 +1,1 @@
-"""B200-native DDPM sampling hot path of music-spectrogram-diffusion."""
+"""H100-native (sm_90a) DDPM sampling hot path of music-spectrogram-diffusion."""

@@ -18,11 +18,11 @@ _CSRC = os.path.join(_HERE, 'csrc')
 _INCLUDE = os.path.join(os.path.dirname(_HERE), 'include')
 LIB_NAME = 'libmsd_b200.so'
 LIB_PATH = os.path.join(_HERE, LIB_NAME)
-SOURCES = ['gemm_tcgen05.cu', 'attention_tcgen05.cu', 'attention_f32.cu', 'elementwise.cu',
+SOURCES = ['gemm_wgmma.cu', 'attention_wgmma.cu', 'attention_f32.cu', 'elementwise.cu',
            'engine.cu']
-HEADERS = ['common.cuh', 'kernels.h']
+HEADERS = ['common.cuh', 'kernels.h', 'wgmma.cuh']
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo',
     '-std=c++17', '-Xcompiler', '-fPIC',
 ]
 
@@ -48,7 +48,7 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-  """Compile csrc/*.cu for sm_100a into the in-tree shared library."""
+  """Compile csrc/*.cu for sm_90a into the in-tree shared library."""
   if not force and not _stale():
     return LIB_PATH
   objdir = os.path.join(_HERE, 'build')
@@ -129,7 +129,6 @@ SYMBOLS = [
     ('msd_bench_gemm', ctypes.c_int, [_I, _I, _I, _I, _I, _I, _I, ctypes.POINTER(ctypes.c_float)]),
     ('msd_bench_attention', ctypes.c_int, [_I, _I, _I, _I, _I, ctypes.POINTER(ctypes.c_float)]),
     ('msd_op_attention', ctypes.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
-    ('msd_op_attention_trace', ctypes.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P]),
     ('msd_op_rmsnorm_film', ctypes.c_int, [_P, _P, _P, _I, _I, _P, _P]),
     ('msd_op_jax_normal', ctypes.c_int, [ctypes.c_uint64, _I, ctypes.c_int64, _P, _P]),
     ('msd_op_jax_bits', ctypes.c_int, [ctypes.c_uint64, _I, ctypes.c_int64, _P, _P]),
@@ -138,7 +137,7 @@ SYMBOLS = [
      [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _I, _I, _P, _P, _P]),
     ('msd_op_attention_f32', ctypes.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
 ]
-ABI_VERSION = 4  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
+ABI_VERSION = 5  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
 
 _lib: Optional[ctypes.CDLL] = None
 

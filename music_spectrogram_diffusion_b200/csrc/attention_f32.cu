@@ -4,7 +4,7 @@
 // msd/layers.py:341-348, rows without an attendable key -> 0 (msd/layers.py:882-902).
 //
 // The reference computes this path in fp32 (gin/models/diffusion/context/t5_base.gin:72); the
-// tensor-core kernel (attention_tcgen05.cu) rounds Q, K, V and P to bf16.  This one is a plain
+// tensor-core kernel (attention_wgmma.cu) rounds Q, K, V and P to bf16.  This one is a plain
 // CUDA-core flash-attention: one CTA per (32 queries, head, batch row), 128 threads, 64-key
 // blocks staged in shared memory, online softmax per query row, thread = 4 rows x 4 columns of
 // the 32 x 64 score / output tiles.  It is the accuracy mode, not the fast path: ~25 TFLOP/s.
@@ -278,7 +278,7 @@ int launch_attention_f32(const AttnF32Args& a, cudaStream_t stream) {
     if (a.splits > 0) {
       splits = a.splits;
     } else {
-      int sms = 148, dev = 0;
+      int sms = 132, dev = 0;
       if (cudaGetDevice(&dev) == cudaSuccess)
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       for (int s = 2; s <= a.max_splits && ctas * (s - 1) < 3 * sms; ++s)

@@ -1,5 +1,5 @@
-// Shared device-side helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM
-// PTX wrappers and UMMA descriptor builders.  Hand-written inline PTX; no CUTLASS.
+// Shared device-side helpers for the sm_90a kernels: mbarrier and TMA PTX
+// wrappers and the wgmma descriptor builder.  Hand-written inline PTX; no CUTLASS.
 #pragma once
 
 #include <cuda.h>
@@ -37,18 +37,6 @@ void set_error(const char* fmt, ...);
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
@@ -112,11 +100,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// generic-proxy writes (st.shared) -> visible to the async proxy (UMMA / TMA reads)
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-
 // ----------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) loads, 2D, completion on an mbarrier
 // ----------------------------------------------------------------------------
@@ -133,261 +116,27 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// TMA store smem -> global (bulk async group completion)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0,
-                                             int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-// TMA reduction smem -> global: global[tile] += smem[tile] (element type of the tensor map; one
-// fp32 add per element at the L2, same rounding as an FADD).  SASS: UTMAREDG.2D.ADD.
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const void* smem_src, int c0,
-                                                  int c1) {
-  asm volatile(
-      "cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-          reinterpret_cast<uint64_t>(m)),
-      "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() {
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {  // smem of all but N groups is reusable
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void tma_store_wait_all() {
-  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
-// Compile-time barrier ids: with the id in a register ptxas must assume that all 16 hardware
-// barriers are used, which limits the kernel to ONE CTA per SM (the SM's 16 barriers are shared by
-// its resident CTAs).
-template <uint32_t kId>
-__device__ __forceinline__ void named_barrier_arrive_c(uint32_t threads) {
-  asm volatile("bar.arrive %0, %1;" ::"n"(kId), "r"(threads) : "memory");
-}
-template <uint32_t kId>
-__device__ __forceinline__ void named_barrier_sync_c(uint32_t threads) {
-  asm volatile("bar.sync %0, %1;" ::"n"(kId), "r"(threads) : "memory");
-}
-__device__ __forceinline__ void named_barrier_arrive(uint32_t id, uint32_t threads) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-__device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-
 // ----------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads, fences
+// wgmma shared-memory matrix descriptors (PTX ISA "asynchronous warpgroup-level matrix
+// shared memory layout / matrix descriptor")
 // ----------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_slot)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread are done.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-
-// ---- CTA-pair (cta_group::2) variants: the two CTAs of a 2-CTA cluster cooperate on one
-// M=256 tile; the even CTA ("leader", cluster rank 0) issues the MMAs for both.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // shared::cluster address -> same offset in the even CTA
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_slot) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_slot)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-// TMA load whose completion bytes are credited to the LEADER CTA's mbarrier (same smem offset).
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m,
-                                                uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)),
-      "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on the barrier at this smem offset in BOTH CTAs of the pair once prior MMAs retire.
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  const uint16_t mask = 0x3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64"
-      " [%0], %1;" ::"r"(smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// Arrive (count 1) on the barrier at this smem offset in the leader (even) CTA.
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask)
-               : "memory");
-}
-
-// TMEM -> registers: each thread reads 32 consecutive 32-bit columns of ITS lane
-// (lane = 32*(warp%4) + laneid).  taddr = (lane_base << 16) | column.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// registers -> TMEM (same lane/column mapping as the load above)
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]),
-        "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]),
-        "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-        "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: PTX ISA "tcgen05 matrix / instruction descriptor")
-// ----------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle, sm_100 version field = 1.
 //   bits [0,14)  start address >> 4
 //   bits [16,30) leading-dim byte offset >> 4
 //   bits [32,46) stride-dim  byte offset >> 4
-//   bits [46,48) version = 1
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-// K-major operand tile [rows][64 bf16] (128-byte rows, TMA SWIZZLE_128B):
-//   8-row groups are 1024 B apart (SBO); LBO is unused for swizzled K-major.
-// MN-major operand tile [k][64 bf16] (128-byte rows indexed by k): 8-k groups
-//   are 1024 B apart (SBO); LBO (stride between 64-wide MN atoms) unused for MN=64.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t sbo_bytes,
-                                                         uint32_t lbo_bytes) {
+//   bits [62,64) layout type: 1 = SWIZZLE_128B
+// K-major operand tile [rows][64 bf16] (128-byte rows, TMA SWIZZLE_128B): 8-row groups are
+//   1024 B apart (SBO); LBO is unused for swizzled K-major; a k-step of 16 elements advances the
+//   start address by 32 B inside the swizzle atom.
+// MN-major operand tile [k][64 bf16] (128-byte rows indexed by k): 8-k groups are 1024 B apart
+//   (SBO); LBO (stride between 64-wide MN atoms) unused for MN = 64; a k-step of 16 advances the
+//   start address by 2048 B.
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-
-// Cheap form for the MMA-issuing thread: the high word of every SWIZZLE_128B descriptor used
-// here is a constant (SBO = 1024 B, version 1, layout type 2) and the low word is
-// (address >> 4) | (LBO 16 B << 16), so stepping through a tile is one 32-bit add per operand
-// instead of rebuilding the 64-bit descriptor (ncu: ~30 uniform-datapath instructions per
-// tcgen05.mma made the small attention MMAs issue-bound).
-constexpr uint32_t kDescHiSw128 = (1024u >> 4) | (1u << 14) | (2u << 29);
-__device__ __forceinline__ uint32_t desc_lo_sw128(uint32_t saddr) {
-  return ((saddr & 0x3FFFFu) >> 4) | (1u << 16);
-}
-__device__ __forceinline__ void umma_bf16_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(kDescHiSw128)
-      : "memory");
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D fmt (1=f32)  [7,10) A fmt (1=bf16)  [10,13) B fmt (1=bf16)
-//   [15] A major (0=K)   [16] B major (0=K,1=MN)  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------

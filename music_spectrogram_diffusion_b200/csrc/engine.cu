@@ -80,14 +80,6 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
                       uint64_t ld, uint32_t box_rows) {
   return make_tmap_2d(out, base, rows, cols, ld, box_rows, 2);
 }
-int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                     uint64_t ld, uint32_t box_rows) {
-  return make_tmap_2d(out, base, rows, cols, ld, box_rows, 4);
-}
-int make_tmap_bf16_2d_half(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                           uint64_t ld, uint32_t box_rows) {
-  return make_tmap_2d(out, base, rows, cols, ld, box_rows, 2, 64);
-}
 
 static int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                         uint64_t ld, uint32_t box_rows, int elem_bytes, int inner_bytes) {
@@ -179,7 +171,7 @@ struct Encoder {
 
 using namespace msd;
 
-// most column tiles a residual projection can have (narrowest CTA-pair tile: 64 columns of d <= 1024)
+// most column tiles a residual projection can have (narrowest tile: 64 columns of d <= 1024)
 static constexpr size_t kSsParts = 16;
 
 struct msd_ctx {
@@ -224,10 +216,8 @@ struct msd_ctx {
   bf16* attn2 = nullptr;   // [B*N, ks*2*hh] outputs of the two cross-attentions (sum_cross_attends)
   float* attn_part_o = nullptr;   // split-KV partials of the cross-attention [B*N*H*8, 64]
   float* attn_part_ml = nullptr;  // [B*N*H*8, 2]
-  uint32_t* attn_flags = nullptr; // tail-mode hand-shake words, one per softmax warp, kept at 0
   float* attn_part_o2 = nullptr;  // second scratch set: sum_cross_attends launches two cross-
   float* attn_part_ml2 = nullptr; //   attentions back to back (PDL lets them overlap)
-  uint32_t* attn_flags2 = nullptr;
   // deferred normalisation (bf16 mode; kernels.h GemmPrep / GemmRowScale): no stand-alone rmsnorm
   // kernels inside the decoder layers
   bool fused_norm = false;
@@ -707,7 +697,7 @@ static int gemm_pos(const bf16* A, int lda, const bf16* B, int ldb, int M, int N
 // `o_width` (bf16 [rows, o_width], acc: [rows, 3 * o_width] = [hi | lo | hi]); head h goes to
 // columns o_col + h*64.
 struct AttnExtra {
-  float* part_o = nullptr; float* part_ml = nullptr; uint32_t* flags = nullptr;
+  float* part_o = nullptr; float* part_ml = nullptr;
   int kv_static = 0, kv_batch_rows = 0, kv_row0 = 0;
 };
 static int attention(const msd_ctx* c, const void* Q, size_t qoff, int ldq, const void* K,
@@ -729,10 +719,13 @@ static int attention(const msd_ctx* c, const void* Q, size_t qoff, int ldq, cons
   AttnArgs a;
   memset(&a, 0, sizeof(a));
   a.kv_static = x.kv_static; a.kv_batch_rows = x.kv_batch_rows; a.kv_row0 = x.kv_row0;
-  a.part_o = x.part_o; a.part_ml = x.part_ml; a.max_splits = 12; a.flags = x.flags;
+  a.part_o = x.part_o; a.part_ml = x.part_ml; a.max_splits = 12;
   {
-    const char* f = getenv("MSD_ATTN_TAIL");  // tuning / test hook: -1 off, 0 auto, n forced
-    a.tail = f ? atoi(f) : 0;
+    // tuning / test hook: n > 0 forces a tail of n key blocks on every attention of the step that
+    // has more than n blocks of 128 keys (the cross-attentions; the self-attention has 2)
+    const char* f = getenv("MSD_ATTN_TAIL");
+    const int t = f ? atoi(f) : 0;
+    a.tail = (t > 0 && t < Lk / 128) ? t : 0;
   }
   a.Q = static_cast<const bf16*>(at(c, Q, qoff)); a.ldq = ldq;
   a.K = static_cast<const bf16*>(at(c, K, koff)); a.ldk = ldk;
@@ -782,7 +775,7 @@ static int cross_attention_block(msd_ctx* c, const DecLayer& w, int l, float* x,
   MSD_TRY(norm_into(c, x, w.ln_cross, R, xn, nullptr, 0, st));
   const size_t kv_off = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;  // elements
   AttnExtra ex;
-  ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml; ex.flags = c->attn_flags;
+  ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml;
   ex.kv_static = 1;
   if (c->cfg.cross_attend_style == 0) {
     MSD_TRY(dense(c, xn, w.cross_q, R, hh, d, epi_qkv(c), c->qc, hh, nullptr, st));
@@ -797,7 +790,7 @@ static int cross_attention_block(msd_ctx* c, const DecLayer& w, int l, float* x,
   MSD_TRY(attention(c, c->qc, 0, 2 * hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh, 2 * hh,
                     c->attn2, 2 * hh, 0, nseg, c->H, N, c->T, c->mask_bits, c->Mkv / 32, st, ex));
   ex.kv_row0 = c->T;
-  ex.part_o = c->attn_part_o2; ex.part_ml = c->attn_part_ml2; ex.flags = c->attn_flags2;
+  ex.part_o = c->attn_part_o2; ex.part_ml = c->attn_part_ml2;
   MSD_TRY(attention(c, c->qc, hh, 2 * hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh, 2 * hh,
                     c->attn2, 2 * hh, hh, nseg, c->H, N, c->C, c->mask_bits + c->T / 32, c->Mkv / 32,
                     st, ex));
@@ -876,7 +869,7 @@ static int decoder_layers_fused(msd_ctx* c, int nseg, int ncross, cudaStream_t s
     a.prep.split_row = split_row;
     a.prep.a = xn; a.prep.lda = d;
     a.prep.ss = ss; a.prep.ss_stride = ss_stride;
-    *parts = d / gemm_pick_pair_bn(M, d);
+    *parts = d / gemm_pick_wide_bn(M, d);
     return launch_gemm(a, st);
   };
   auto row_scale = [&](GemmArgs& a, const float* lo, int parts_lo, const float* hi, int parts_hi,
@@ -910,7 +903,7 @@ static int decoder_layers_fused(msd_ctx* c, int nseg, int ncross, cudaStream_t s
       MSD_TRY(launch_gemm(a, st));
       const size_t kv_off = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;
       AttnExtra ex;
-      ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml; ex.flags = c->attn_flags;
+      ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml;
       ex.kv_static = 1;
       if (nsrc == 1) {
         MSD_TRY(attention(c, c->qc, 0, hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh, 2 * hh,
@@ -924,7 +917,7 @@ static int decoder_layers_fused(msd_ctx* c, int nseg, int ncross, cudaStream_t s
                           2 * hh, c->attn2, 2 * hh, 0, ncross, c->H, N, c->T, c->mask_bits, c->Mkv / 32,
                           st, ex));
         ex.kv_row0 = c->T;
-        ex.part_o = c->attn_part_o2; ex.part_ml = c->attn_part_ml2; ex.flags = c->attn_flags2;
+        ex.part_o = c->attn_part_o2; ex.part_ml = c->attn_part_ml2;
         MSD_TRY(attention(c, c->qc, hh, 2 * hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh,
                           2 * hh, c->attn2, 2 * hh, hh, ncross, c->H, N, c->C, c->mask_bits + c->T / 32,
                           c->Mkv / 32, st, ex));
@@ -1090,7 +1083,7 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   MSD_CUDA_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   MSD_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-  MSD_REQUIRE(prop.major == 10, "msd_create: device %d is sm_%d%d; this library is sm_100a only",
+  MSD_REQUIRE(prop.major == 9, "msd_create: device %d is sm_%d%d; this library is sm_90a only",
               device, prop.major, prop.minor);
   MSD_TRY(gemm_configure());
   MSD_TRY(attention_configure());
@@ -1114,9 +1107,8 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   do {
     {
       // Opt-in experiment (MSD_TWO_STREAMS=1): conditional / unconditional passes as two concurrent
-      // kernel chains.  Measured on B200 at B = 8: 1080 vs 1123 frames/s for the single chain
-      // (every GEMM / attention CTA owns a whole SM's shared memory, so the chains mostly
-      // time-share SMs, and the half-height GEMMs are less efficient) -> off by default.
+      // kernel chains.  Every GEMM / attention CTA owns a whole SM's shared memory, so the chains
+      // mostly time-share SMs, and the half-height GEMMs are less efficient -> off by default.
       const char* ts = getenv("MSD_TWO_STREAMS");
       c->two_streams = (ts && ts[0] == '1') && !c->acc;
     }
@@ -1138,26 +1130,13 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
     if ((rc = A.alloc(&c->qc, BN * c->hh * (cfg->cross_attend_style == 1 ? 2 : 1) * qe))) break;
     if (cfg->cross_attend_style == 1 && (rc = A.alloc(&c->attn2, BN * 2 * c->hh * ks))) break;
     constexpr int kMaxSplits = 12;
-    const size_t nflags = attention_flag_words(c->Bmax, c->H, c->N, kMaxSplits) + 64;
     const size_t npart = attention_workspace_floats(c->Bmax, c->H, c->N, kMaxSplits);
     if ((rc = A.alloc(&c->attn_part_o, npart))) break;
     if ((rc = A.alloc(&c->attn_part_ml, BN * c->H * kMaxSplits * 2))) break;
-    if ((rc = A.alloc(&c->attn_flags, nflags))) break;
-    if (cudaMemset(c->attn_flags, 0, nflags * sizeof(uint32_t)) != cudaSuccess) {
-      set_error("msd_create: cudaMemset failed");
-      rc = -2;
-      break;
-    }
-    c->attn_part_o2 = c->attn_part_o; c->attn_part_ml2 = c->attn_part_ml; c->attn_flags2 = c->attn_flags;
+    c->attn_part_o2 = c->attn_part_o; c->attn_part_ml2 = c->attn_part_ml;
     if (cfg->cross_attend_style == 1) {
       if ((rc = A.alloc(&c->attn_part_o2, npart))) break;
       if ((rc = A.alloc(&c->attn_part_ml2, BN * c->H * kMaxSplits * 2))) break;
-      if ((rc = A.alloc(&c->attn_flags2, nflags))) break;
-      if (cudaMemset(c->attn_flags2, 0, nflags * sizeof(uint32_t)) != cudaSuccess) {
-        set_error("msd_create: cudaMemset failed");
-        rc = -2;
-        break;
-      }
     }
     {
       // MSD_FUSED_NORM=0: tuning / test hook, keeps the stand-alone rmsnorm kernels
@@ -1554,7 +1533,7 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
   memset(&ga, 0, sizeof(ga));
   ga.A = a; ga.B = b; ga.M = M; ga.N = N; ga.K = K; ga.lda = K; ga.ldb = K;
   ga.epilogue = epilogue; ga.out = o; ga.ldo = (epilogue == EPI_GATED_GELU) ? N / 2 : N;
-  ga.resid = (variant == 1) ? r : o;  // CTA-pair kernel: in place (TMA reduce-add), like the engine
+  ga.resid = (variant == 1) ? r : o;  // default variant: in place, like the engine
   ga.variant = variant; ga.block_n = block_n;
   cudaStream_t st = nullptr;
   MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
@@ -1620,17 +1599,13 @@ int msd_bench_attention(int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32
   TempBufs tb;
   bf16 *qb, *kb, *vb, *ob;
   float *tmp, *po, *pml;
-  uint32_t* fl;
   const size_t nq = static_cast<size_t>(nb) * Lq * w, nk = static_cast<size_t>(nb) * Lk * w;
   MSD_TRY(tb.get(&qb, nq)); MSD_TRY(tb.get(&kb, nk)); MSD_TRY(tb.get(&vb, nk)); MSD_TRY(tb.get(&ob, nq));
   MSD_TRY(tb.get(&tmp, nk));
   MSD_TRY(tb.get(&po, attention_workspace_floats(nb, heads, Lq, 12)));
   MSD_TRY(tb.get(&pml, static_cast<size_t>(nb) * Lq * heads * 12 * 2));
-  const size_t nfl = attention_flag_words(nb, heads, Lq, 12);
-  MSD_TRY(tb.get(&fl, nfl));
   cudaStream_t st = nullptr;
   MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  MSD_CUDA_CHECK(cudaMemsetAsync(fl, 0, nfl * sizeof(uint32_t), st));
   // N(0,1) * 0.3-ish values through the jax generator (any bounded values would do)
   MSD_TRY(launch_jax_normal(1u, 2u, static_cast<long long>(nk), tmp, st));
   MSD_TRY(launch_f32_to_bf16(tmp, kb, static_cast<long long>(nk), st));
@@ -1640,7 +1615,7 @@ int msd_bench_attention(int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32
   memset(&aa, 0, sizeof(aa));
   aa.Q = qb; aa.ldq = w; aa.K = kb; aa.ldk = w; aa.V = vb; aa.ldv = w; aa.O = ob; aa.ldo = w;
   aa.nbatch = nb; aa.heads = heads; aa.Lq = Lq; aa.Lk = Lk;
-  aa.part_o = po; aa.part_ml = pml; aa.max_splits = 12; aa.flags = fl; aa.kv_static = 1;
+  aa.part_o = po; aa.part_ml = pml; aa.max_splits = 12; aa.kv_static = 1;
   {
     const char* f = getenv("MSD_ATTN_SPLITS");
     aa.splits = f ? atoi(f) : 0;
@@ -1669,12 +1644,6 @@ int msd_bench_attention(int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32
 
 int msd_op_attention(const float* q, const float* k, const float* v, const int32_t* key_mask,
                      int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, float* out, void* stream) {
-  return msd_op_attention_trace(q, k, v, key_mask, nb, heads, Lq, Lk, out, nullptr, stream);
-}
-
-int msd_op_attention_trace(const float* q, const float* k, const float* v,
-                           const int32_t* key_mask, int32_t nb, int32_t heads, int32_t Lq,
-                           int32_t Lk, float* out, int64_t* trace, void* stream) {
   MSD_REQUIRE(q && k && v && out, "msd_op_attention: null argument");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int w = heads * 64;
@@ -1697,20 +1666,15 @@ int msd_op_attention_trace(const float* q, const float* k, const float* v,
     memset(&aa, 0, sizeof(aa));
     aa.Q = qb; aa.ldq = w; aa.K = kb; aa.ldk = w; aa.V = vb; aa.ldv = w; aa.O = ob; aa.ldo = w;
     aa.nbatch = nb; aa.heads = heads; aa.Lq = Lq; aa.Lk = Lk; aa.mask_bits = bits;
-    aa.mask_stride_words = Lk / 32; aa.trace = reinterpret_cast<long long*>(trace);
+    aa.mask_stride_words = Lk / 32;
     float *po = nullptr, *pml = nullptr;
     MSD_TRY(tb.get(&po, attention_workspace_floats(nb, heads, Lq, 12)));
     MSD_TRY(tb.get(&pml, static_cast<size_t>(nb) * Lq * heads * 12 * 2));
     aa.part_o = po; aa.part_ml = pml; aa.max_splits = 12;
-    uint32_t* fl = nullptr;
-    const size_t nfl = attention_flag_words(nb, heads, Lq, 12);
-    MSD_TRY(tb.get(&fl, nfl));
-    MSD_CUDA_CHECK(cudaMemsetAsync(fl, 0, nfl * sizeof(uint32_t), st));
-    aa.flags = fl;
     {
       const char* f = getenv("MSD_ATTN_SPLITS");  // test hook: force a split count
       aa.splits = f ? atoi(f) : 0;
-      const char* t = getenv("MSD_ATTN_TAIL");    // test hook: force a tail length (-1 = off)
+      const char* t = getenv("MSD_ATTN_TAIL");    // test hook: force a tail length
       aa.tail = t ? atoi(t) : 0;
     }
     MSD_TRY(launch_attention(aa, st));
@@ -1816,7 +1780,7 @@ int msd_op_dense_deferred_norm(const float* a, const float* w_out, const float* 
   bf16 *ab = nullptr, *wo = nullptr, *opnd = nullptr, *w2p = nullptr, *yb = nullptr;
   float* ss = nullptr;
   int* step0 = nullptr;
-  const int bn1 = block_n1 ? block_n1 : gemm_pick_pair_bn(M, d);
+  const int bn1 = block_n1 ? block_n1 : gemm_pick_wide_bn(M, d);
   MSD_REQUIRE(bn1 > 0 && d % bn1 == 0, "msd_op_dense_deferred_norm: block_n1 must divide d");
   const int parts = d / bn1;
   MSD_TRY(tb.get(&ab, static_cast<size_t>(M) * K));

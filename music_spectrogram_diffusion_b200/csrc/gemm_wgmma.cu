@@ -1,0 +1,442 @@
+// bf16 GEMM on the Hopper tensor cores: D[M,N] = A[M,K] * B[N,K]^T.
+//
+// One CTA per 128 x BN output tile, three warpgroups:
+//   warpgroup 0 (one lane)  TMA producer: cp.async.bulk.tensor 2D tiles (SWIZZLE_128B) into a
+//                           STAGES-deep smem ring, completion on `full` mbarriers; its register
+//                           allowance goes to the consumers (setmaxnreg)
+//   warpgroups 1, 2         consumers: 64 rows each, wgmma.mma_async m64 x nBN x k16 straight from
+//                           the ring (fp32 accumulator fragment in registers), one MMA group kept
+//                           in flight while the previous ring slot is handed back (`empty`), then
+//                           the fused epilogue (residual / gated-GELU / position-add / deferred
+//                           normalisation) from the accumulator fragment: a quad of lanes owns 8
+//                           consecutive columns of a row, so every store covers whole 32-byte
+//                           sectors (fp32) or 16-byte half sectors (bf16)
+//
+// Replaces the XLA dot_general lowering of DenseGeneral (msd/layers.py:397-442) for every
+// projection on the hot path (SURVEY §2.2 K2, K4, K5, K6, K8, K9).
+#include <stdlib.h>
+
+#include "common.cuh"
+#include "kernels.h"
+#include "wgmma.cuh"
+
+namespace msd {
+
+namespace {
+
+constexpr int BLOCK_M = 128;
+constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle atom row
+constexpr int MMA_K = 16;
+constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;
+constexpr int GEMM_THREADS = 384;
+
+__host__ __device__ inline bool epi_is_bf16_out(int e) {
+  return e == EPI_BF16 || e == EPI_GATED_GELU || e == EPI_GATED_GELU_SPLIT3;
+}
+
+// exact-tanh GELU of the fp32-accurate mode (flax.linen.gelu(approximate=True))
+__device__ __forceinline__ float gelu_tanh_exact(float x) {
+  const float k0 = 0.7978845608028654f;
+  return 0.5f * x * (1.0f + tanhf(k0 * (x + 0.044715f * x * x * x)));
+}
+
+struct GemmDev {
+  int M, N, K;
+  int epilogue;
+  void* out;
+  int ldo;
+  const float* resid;
+  const float* pos;
+  int pos_rows;
+  const int* pos_shift;
+  int dup_rows;
+  // debugging (MSD_GEMM_TRACE with msd_bench_gemm): per CTA 8 int64 -- smid, globaltimer at entry /
+  // exit, total clock64 cycles, then clock64 offsets from entry of: set-up done, main loop entered,
+  // accumulator complete and dependency wait returned, last store issued (first 512 CTAs)
+  long long* trace;
+  GemmPrep prep;       // EPI_RESID_PREP
+  GemmRowScale rs;     // row scale + bias on EPI_BF16 / EPI_GATED_GELU
+  const int* step;
+};
+
+template <int BN>
+struct GemmCfg {
+  static constexpr int B_STAGE_BYTES = BN * BLOCK_K * 2;
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+  static constexpr int STAGE_BUDGET = 200 * 1024;
+  static constexpr int STAGES = STAGE_BUDGET / STAGE_BYTES > 6 ? 6 : STAGE_BUDGET / STAGE_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/ + 1024 /*align*/;
+};
+
+template <int BN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                       const __grid_constant__ CUtensorMap tmap_b, const GemmDev p) {
+  using Cfg = GemmCfg<BN>;
+  constexpr int STAGES = Cfg::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + STAGES * A_STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + STAGES * Cfg::B_STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
+
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  const int n0 = blockIdx.x * BN;
+  const int m0 = blockIdx.y * BLOCK_M;
+  const int num_kb = p.K / BLOCK_K;
+  const int cta = blockIdx.y * gridDim.x + blockIdx.x;
+  long long* trc = (p.trace != nullptr && threadIdx.x == 128 && cta < 512) ? p.trace + cta * 8 : nullptr;
+  long long t_entry = 0;
+  if (trc) {
+    uint32_t smid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    t_entry = clock64();
+    trc[0] = smid; trc[1] = t;
+  }
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+#pragma unroll
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (trc) trc[4] = clock64() - t_entry;
+
+  griddep_launch_dependents();
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
+      // The weight (B) tiles do not depend on the previous kernel: the first ring-full of them is
+      // requested BEFORE griddepcontrol.wait so the fetch overlaps the predecessor's tail.
+      const int prefetched = num_kb < STAGES ? num_kb : STAGES;
+      for (int kb = 0; kb < prefetched; ++kb) {
+        mbar_arrive_expect_tx(&full_bar[kb], Cfg::STAGE_BYTES);
+        tma_load_2d(sB + kb * Cfg::B_STAGE_BYTES, &tmap_b, &full_bar[kb], kb * BLOCK_K, n0);
+      }
+      griddep_wait();
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % STAGES;
+        const uint32_t ph = (kb / STAGES) & 1;
+        if (kb < prefetched) {  // slot was armed and its B tile requested above
+          tma_load_2d(sA + s * A_STAGE_BYTES, &tmap_a, &full_bar[s], kb * BLOCK_K, m0);
+          continue;
+        }
+        mbar_wait(&empty_bar[s], ph ^ 1u);
+        mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+        tma_load_2d(sA + s * A_STAGE_BYTES, &tmap_a, &full_bar[s], kb * BLOCK_K, m0);
+        tma_load_2d(sB + s * Cfg::B_STAGE_BYTES, &tmap_b, &full_bar[s], kb * BLOCK_K, n0);
+      }
+    }
+    return;
+  }
+
+  // ------------------------------ consumers ------------------------------
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = (warp >> 2) - 1;  // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
+  const int tid = threadIdx.x & 127;
+  float acc[BN / 2];
+  if (trc) trc[5] = clock64() - t_entry;
+  {
+    const uint64_t da0 = make_smem_desc_sw128(smem_u32(sA) + wg * 64 * 128);
+    const uint64_t db0 = make_smem_desc_sw128(smem_u32(sB));
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int s = kb % STAGES;
+      mbar_wait(&full_bar[s], (kb / STAGES) & 1);
+      const uint64_t da = da0 + static_cast<uint64_t>(s * (A_STAGE_BYTES >> 4));
+      const uint64_t db = db0 + static_cast<uint64_t>(s * (Cfg::B_STAGE_BYTES >> 4));
+      wgmma_fence_regs(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / MMA_K; ++k)
+        WgmmaSS<BN>::mma(acc, da + k * 2, db + k * 2, (kb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();  // the MMAs of the previous k-block have retired: its slot is free
+      if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[(kb - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+  }
+  griddep_wait();  // residual reads / output writes come after the predecessor is complete
+  if (trc) trc[6] = clock64() - t_entry;
+
+  // ---------------- epilogue from the accumulator fragment ----------------
+  const int q = lane & 3;
+  const int row_first = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row_first + 8 * h;
+    if (row >= p.M) continue;
+    // deferred normalisation, consumer side: this row's scale (and the bias row below)
+    float inv_r = 1.0f;
+    const float* bias = nullptr;
+    if (p.rs.ss_lo != nullptr) {
+      const bool lo = row < p.rs.split_row;
+      const float* ssp = (lo ? p.rs.ss_lo : p.rs.ss_hi) + row;
+      const int parts = lo ? p.rs.parts_lo : p.rs.parts_hi;
+      float ss = 0.f;
+      for (int t = 0; t < parts; ++t) ss += ssp[static_cast<size_t>(t) * p.rs.ss_stride];
+      inv_r = rsqrtf(ss * p.rs.inv_d + 1e-6f);
+      if (p.rs.col_bias != nullptr)
+        bias = p.rs.col_bias + (p.step != nullptr ? *p.step : 0) * p.rs.bias_step_stride;
+    }
+    if (p.epilogue == EPI_GATED_GELU || p.epilogue == EPI_GATED_GELU_SPLIT3) {
+      bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
+      const int F = p.N / 2;
+#pragma unroll
+      for (int c = 0; c < BN; c += 64) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int jr = c / 8 + jj, jg = jr + 4;
+          float r0 = acc[4 * jr + 2 * h], r1 = acc[4 * jr + 2 * h + 1];
+          float g0 = acc[4 * jg + 2 * h], g1 = acc[4 * jg + 2 * h + 1];
+          if (p.rs.ss_lo != nullptr) {
+            r0 *= inv_r; r1 *= inv_r; g0 *= inv_r; g1 *= inv_r;
+            if (bias != nullptr) {
+              const float2 br = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * jr + 2 * q));
+              const float2 bg = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * jg + 2 * q));
+              r0 += br.x; r1 += br.y; g0 += bg.x; g1 += bg.y;
+            }
+          }
+          const int oc = (n0 + c) / 2 + 8 * jj + 2 * q;
+          if (p.epilogue == EPI_GATED_GELU) {
+            *reinterpret_cast<uint32_t*>(out + oc) = pack_bf16(gelu_tanh(r0) * g0, gelu_tanh(r1) * g1);
+          } else {
+            // fp32-accurate mode: exact tanh, result kept to ~16 mantissa bits as [hi | lo | hi]
+            const float v0 = gelu_tanh_exact(r0) * g0, v1 = gelu_tanh_exact(r1) * g1;
+            const uint32_t hi = pack_bf16(v0, v1);
+            const uint32_t lo = pack_bf16(v0 - __bfloat162float(__float2bfloat16_rn(v0)),
+                                          v1 - __bfloat162float(__float2bfloat16_rn(v1)));
+            *reinterpret_cast<uint32_t*>(out + oc) = hi;
+            *reinterpret_cast<uint32_t*>(out + F + oc) = lo;
+            *reinterpret_cast<uint32_t*>(out + 2 * F + oc) = hi;
+          }
+        }
+      }
+    } else if (p.epilogue == EPI_BF16) {
+      bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * q;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (p.rs.ss_lo != nullptr) {
+          v0 *= inv_r; v1 *= inv_r;
+          if (bias != nullptr) {
+            const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
+            v0 += b2.x; v1 += b2.y;
+          }
+        }
+        *reinterpret_cast<uint32_t*>(out + col) = pack_bf16(v0, v1);
+      }
+    } else if (p.epilogue == EPI_RESID_PREP) {
+      // deferred normalisation, producer side: x = acc + residual (in place), the next GEMM's
+      // operand bf16(x * g) and this tile's share of the row's sum of squares
+      float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
+      bf16* arow = p.prep.a + static_cast<size_t>(row) * p.prep.lda;
+      const long long st = p.step != nullptr ? *p.step : 0;
+      const float* gvec = row < p.prep.split_row ? p.prep.g_lo + st * p.prep.g_lo_step_stride
+                                                 : p.prep.g_hi + st * p.prep.g_hi_step_stride;
+      float ssum = 0.f;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * q;
+        const float2 x = *reinterpret_cast<const float2*>(out + col);
+        const float2 g = __ldg(reinterpret_cast<const float2*>(gvec + col));
+        const float v0 = acc[4 * j + 2 * h] + x.x, v1 = acc[4 * j + 2 * h + 1] + x.y;
+        ssum = fmaf(v0, v0, ssum);
+        ssum = fmaf(v1, v1, ssum);
+        *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+        *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g.x, v1 * g.y);
+      }
+      ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
+      ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
+      if (q == 0) p.prep.ss[static_cast<size_t>(n0 / BN) * p.prep.ss_stride + row] = ssum;
+    } else {
+      float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
+      const float* add = nullptr;  // row added to the accumulator
+      if (p.epilogue == EPI_RESID_F32) {
+        add = p.resid + static_cast<size_t>(row) * p.ldo;
+      } else if (p.epilogue == EPI_POS_F32) {
+        const int seq = row / p.pos_rows;
+        int pr = row - seq * p.pos_rows;
+        if (p.pos_shift != nullptr) {
+          pr -= p.pos_shift[seq];
+          if (pr < 0) pr += p.pos_rows;
+        }
+        add = p.pos + static_cast<size_t>(pr) * p.N;
+      }
+      const bool dup = p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * q;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (add != nullptr) {
+          const float2 x = *reinterpret_cast<const float2*>(add + col);
+          v0 += x.x; v1 += x.y;
+        }
+        *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+        if (dup)
+          *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
+              make_float2(v0, v1);
+      }
+    }
+  }
+  if (trc) {
+    long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    trc[2] = t;
+    trc[7] = clock64() - t_entry;
+    trc[3] = trc[7];
+  }
+}
+
+// SMs of the current device (132 on H100 SXM): one CTA is resident per SM.
+static int gemm_sm_count() {
+  static thread_local int cached_dev = -1, cached = 0;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (dev != cached_dev) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    cached = n;
+    cached_dev = dev;
+  }
+  return cached;
+}
+
+template <int BN>
+int launch_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& d, cudaStream_t st) {
+  using Cfg = GemmCfg<BN>;
+  static_assert(Cfg::SMEM_BYTES <= 227 * 1024 && Cfg::STAGES >= 3, "smem budget");
+  dim3 grid(d.N / BN, (d.M + BLOCK_M - 1) / BLOCK_M);
+  ProfScope prof(KC_GEMM, 2.0 * d.M * d.N * d.K,
+                 2.0 * (static_cast<double>(d.M) * d.K + static_cast<double>(d.N) * d.K) +
+                     4.0 * d.M * d.N, st);
+  MSD_CUDA_CHECK(launch_kernel(gemm_bf16_wgmma_kernel<BN>, grid, dim3(GEMM_THREADS), Cfg::SMEM_BYTES,
+                               st, ta, tb, d));
+  ++g_launch_count;
+  return 0;
+}
+
+template <int BN>
+int configure_bn() {
+  MSD_CUDA_CHECK(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN>,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      GemmCfg<BN>::SMEM_BYTES));
+  return 0;
+}
+
+}  // namespace
+
+int gemm_configure() {
+  if (int rc = configure_bn<64>()) return rc;
+  if (int rc = configure_bn<96>()) return rc;
+  if (int rc = configure_bn<128>()) return rc;
+  if (int rc = configure_bn<192>()) return rc;
+  return configure_bn<256>();
+}
+
+// Tile width of the default variant: the widest tile re-reads the least of A and B per FLOP, unless
+// it leaves SMs idle that a narrower tiling would use: among the widths whose tile count fits the
+// SMs (one CTA each), take the one with the most tiles.
+int gemm_pick_wide_bn(int M, int N) {
+  const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
+  const int widths[4] = {256, 192, 128, 64};
+  const int conc = gemm_sm_count();
+  int best = 0, best_tiles = 0;
+  for (int i = 0; i < 4; ++i) {
+    const int bn = widths[i];
+    if (N % bn != 0) continue;
+    const int tiles = m_tiles * (N / bn);
+    if (best == 0) { best = bn; best_tiles = tiles; continue; }   // widest dividing width
+    if (best_tiles < conc && tiles <= conc && tiles > best_tiles) { best = bn; best_tiles = tiles; }
+  }
+  return best;
+}
+
+// Tile width of variant 1: power-of-two widths only, a wider tile once it fills every SM.
+int gemm_pick_block_n(int M, int N) {
+  const int mt = (M + BLOCK_M - 1) / BLOCK_M;
+  const int sms = gemm_sm_count();
+  if (N % 256 == 0 && mt * (N / 256) >= 2 * sms) return 256;
+  if (N % 128 == 0 && mt * (N / 128) >= sms) return 128;
+  if (N % 64 == 0) return 64;
+  if (N % 128 == 0) return 128;
+  return 0;
+}
+
+int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
+  static int configured = gemm_configure();
+  if (configured != 0) return configured;
+  MSD_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "gemm: empty problem M=%d N=%d K=%d", a.M, a.N, a.K);
+  MSD_REQUIRE(a.K % BLOCK_K == 0, "gemm: K=%d must be a multiple of %d", a.K, BLOCK_K);
+  MSD_REQUIRE(a.M % BLOCK_M == 0, "gemm: M=%d must be a multiple of %d", a.M, BLOCK_M);
+  static const int forced_variant = [] {
+    const char* e = getenv("MSD_GEMM_VARIANT");  // debugging aid: 1 forces variant 1's tile choice
+    return e ? atoi(e) : 0;
+  }();
+  const bool wide = (forced_variant ? forced_variant : a.variant) != 1;
+  int bn = a.block_n ? a.block_n
+                     : (wide ? gemm_pick_wide_bn(a.M, a.N) : gemm_pick_block_n(a.M, a.N));
+  MSD_REQUIRE(bn == 64 || bn == 128 || bn == 256 || (wide && bn == 192) ||
+                  (wide && bn == 96 && !epi_is_bf16_out(a.epilogue)),
+              "gemm: N=%d has no valid tile width (block_n %d)", a.N, bn);
+  MSD_REQUIRE(a.N % bn == 0, "gemm: N=%d not a multiple of block_n=%d", a.N, bn);
+  MSD_REQUIRE(a.ldo % 8 == 0, "gemm: ldo=%d must be a multiple of 8", a.ldo);
+
+  CUtensorMap ta, tb;
+  if (a.tmap_a) {
+    ta = *a.tmap_a;
+  } else if (int rc = make_tmap_bf16_2d(&ta, a.A, a.M, a.K, a.lda, BLOCK_M)) {
+    return rc;
+  }
+  if (a.tmap_b) {
+    tb = *a.tmap_b;
+  } else if (int rc = make_tmap_bf16_2d(&tb, a.B, a.N, a.K, a.ldb, bn)) {
+    return rc;
+  }
+  GemmDev d;
+  d.M = a.M; d.N = a.N; d.K = a.K;
+  d.epilogue = a.epilogue;
+  d.out = a.out; d.ldo = a.ldo;
+  d.resid = a.resid; d.pos = a.pos; d.pos_rows = a.pos_rows > 0 ? a.pos_rows : 1;
+  d.pos_shift = a.pos_shift; d.dup_rows = a.dup_rows;
+  d.trace = a.trace;
+  d.prep = a.prep; d.rs = a.rs; d.step = a.step;
+  if (a.epilogue == EPI_RESID_F32)
+    MSD_REQUIRE(a.resid != nullptr, "gemm: EPI_RESID_F32 needs the residual");
+  if (a.epilogue == EPI_RESID_PREP) {
+    MSD_REQUIRE(a.resid != nullptr && a.resid == a.out, "gemm: EPI_RESID_PREP works in place (out == resid)");
+    MSD_REQUIRE(a.prep.a && a.prep.ss && a.prep.g_lo && a.prep.g_hi && a.prep.lda % 8 == 0 &&
+                    a.prep.ss_stride >= a.M,
+                "gemm: EPI_RESID_PREP needs prep.a / ss / g_lo / g_hi (lda %% 8 == 0, ss_stride >= M)");
+    MSD_REQUIRE(a.step != nullptr || (a.prep.g_lo_step_stride == 0 && a.prep.g_hi_step_stride == 0),
+                "gemm: step-dependent column scales need the device step index");
+  }
+  if (a.rs.ss_lo != nullptr) {
+    MSD_REQUIRE(a.epilogue == EPI_BF16 || a.epilogue == EPI_GATED_GELU,
+                "gemm: the row scale applies to the bf16 and gated epilogues only");
+    MSD_REQUIRE(a.rs.ss_hi != nullptr && a.rs.parts_lo > 0 && a.rs.parts_hi > 0 && a.rs.inv_d > 0.f,
+                "gemm: incomplete row-scale description");
+    MSD_REQUIRE(a.step != nullptr || a.rs.col_bias == nullptr || a.rs.bias_step_stride == 0,
+                "gemm: a step-dependent bias row needs the device step index");
+  }
+  switch (bn) {
+    case 64: return launch_bn<64>(ta, tb, d, stream);
+    case 96: return launch_bn<96>(ta, tb, d, stream);
+    case 128: return launch_bn<128>(ta, tb, d, stream);
+    case 192: return launch_bn<192>(ta, tb, d, stream);
+    default: return launch_bn<256>(ta, tb, d, stream);
+  }
+}
+
+}  // namespace msd

@@ -1,4 +1,4 @@
-// Host-side launcher prototypes for the sm_100a kernels (internal to libmsd_b200.so).
+// Host-side launcher prototypes for the sm_90a kernels (internal to libmsd_b200.so).
 #pragma once
 
 #include <cuda.h>
@@ -67,16 +67,10 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
 // box = [box_rows, 64 cols] (128-byte inner extent), SWIZZLE_128B.
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
                       uint64_t ld, uint32_t box_rows);
-// Same for fp32 with box = [box_rows, 32 cols] (128-byte inner extent), SWIZZLE_128B.
-int make_tmap_f32_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                     uint64_t ld, uint32_t box_rows);
-// bf16 with box = [box_rows, 32 cols] (64-byte inner extent), SWIZZLE_64B.
-int make_tmap_bf16_2d_half(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                           uint64_t ld, uint32_t box_rows);
 
 // ---------------------------------------------------------------------------
 // GEMM: D[M,N] = A[M,K] * B[N,K]^T, bf16 operands (both K-major), fp32 accumulate
-// in TMEM (tcgen05.mma), TMA-fed smem ring, warp-specialised.
+// in registers (wgmma.mma_async), TMA-fed smem ring, warp-specialised.
 // ---------------------------------------------------------------------------
 enum GemmEpilogue : int {
   EPI_BF16 = 0,        // out bf16 [M, ldo] = acc
@@ -87,8 +81,8 @@ enum GemmEpilogue : int {
                        //   optionally duplicated to out[r + dup_rows]
   EPI_GATED_GELU_SPLIT3 = 5,  // fp32-accurate mode: g = gelu(acc[0:32]) * acc[32:64] with the exact
                               //   tanh, written as bf16 [M, 3 * N/2] = [hi(g) | lo(g) | hi(g)]
-                              //   (the A operand of a 3 x bf16 split-precision GEMM); CTA-pair kernel
-  EPI_RESID_PREP = 6,  // deferred normalisation, producer side (CTA-pair kernel; out == resid):
+                              //   (the A operand of a 3 x bf16 split-precision GEMM)
+  EPI_RESID_PREP = 6,  // deferred normalisation, producer side (out == resid):
                        //   x = acc + resid (f32, in place); prep.a[r, :] = bf16(x[r, :] * g(r)[:])
                        //   with g = prep.g_lo for r < prep.split_row else prep.g_hi; and
                        //   prep.ss[tile_n, r] = sum over the tile's columns of x^2
@@ -137,9 +131,10 @@ struct GemmArgs {
   const CUtensorMap* tmap_a;
   const CUtensorMap* tmap_b;
   int block_n;           // 0 = auto
-  int variant;           // 0 = CTA-pair persistent kernel (default), 1 = single-CTA kernel
-  long long* trace;      // debugging: per-CTA stamps of the CTA-pair kernel (8 int64 per CTA), or null
-  // deferred normalisation (CTA-pair kernel): prep.a != null with EPI_RESID_PREP; rs.ss_lo != null
+  int variant;           // tile-width choice: 0 = widest that fills the SMs (default, 96 / 192 allowed),
+                         // 1 = power-of-two widths only
+  long long* trace;      // debugging: per-CTA stamps (8 int64 per CTA, first 512 CTAs), or null
+  // deferred normalisation: prep.a != null with EPI_RESID_PREP; rs.ss_lo != null
   // with EPI_BF16 / EPI_GATED_GELU; `step` is the device step index the strides multiply
   GemmPrep prep;
   GemmRowScale rs;
@@ -149,7 +144,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream);
 int gemm_configure();  // opt in to the kernels' dynamic shared memory sizes (idempotent)
 // Box rows the A / B maps must be built with for a given block_n choice.
 int gemm_pick_block_n(int M, int N);
-int gemm_pick_pair_bn(int M, int N);
+int gemm_pick_wide_bn(int M, int N);
 
 // ---------------------------------------------------------------------------
 // Attention: O = softmax(Q K^T + keymask) V, no 1/sqrt(d), head_dim 64.
@@ -165,15 +160,14 @@ struct AttnArgs {
   int nbatch, heads, Lq, Lk;
   const uint32_t* mask_bits; int mask_stride_words;
   const CUtensorMap* tmap_q; const CUtensorMap* tmap_k; const CUtensorMap* tmap_v;
-  long long* trace;  // debugging: per-block clock64 stamps of CTA (0,0,0), see attention kernel
   // split-KV workspace (optional): part_o [attention_workspace_floats(..)] f32, part_ml
   // [rows*heads*max_splits*2] f32; splits 0 = choose automatically (attention_pick_splits),
   // capped by max_splits.
   float* part_o; float* part_ml; int splits; int max_splits;
-  // in-kernel merges (tail mode of the 128-key instance, owner merge of the 64-key instance) need
-  // part_o / part_ml and a zeroed flags array of attention_flag_words(..) words:
-  // tail 0 = choose automatically (attention_pick_tail), > 0 = forced, < 0 = off.
-  uint32_t* flags; int tail;
+  // tail split of an otherwise unsplit launch of the 128-key instance (needs the workspace):
+  // tail > 0 = the last `tail` key blocks go to a second (short) CTA per tile, merged by the
+  // combine kernel; <= 0 = none.
+  int tail;
   // K, V and mask_bits were written well before the preceding kernel (safe to read ahead of the
   // programmatic-dependency wait): true for the cross-attention over the per-segment K/V cache.
   int kv_static;
@@ -181,11 +175,9 @@ struct AttnArgs {
   // (kv_batch_rows 0 = Lk): lets one source of a concatenated [tokens | context] cache be attended.
   int kv_batch_rows, kv_row0;
 };
-// workspace sizing for part_o (floats) and flags (words) of a launch with up to max_splits splits
+// workspace sizing for part_o (floats) of a launch with up to max_splits splits
 size_t attention_workspace_floats(int nbatch, int heads, int Lq, int max_splits);
-size_t attention_flag_words(int nbatch, int heads, int Lq, int max_splits);
 int attention_pick_splits(int nbatch, int heads, int Lq, int Lk);
-int attention_pick_tail(int nbatch, int heads, int Lq, int Lk);
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
 int attention_configure();
 

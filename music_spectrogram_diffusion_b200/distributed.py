@@ -7,7 +7,7 @@ Two partitionings of the reference's serve path (SURVEY §8e):
   * one song (config 5): segment k+1's context is segment k's FINAL mel
     (msd/beam/evaluation.py:179-223, colab ipynb:895-935), so the chain is strictly serial.
     `synthesize_song` relays the chain round-robin over the ranks and hands the 128 KB mel
-    GPU-to-GPU with send/recv (NCCL over NVLink on a B200 box, gloo in the CPU tests) instead of
+    GPU-to-GPU with send/recv (NCCL over NVLink on an H100 box, gloo in the CPU tests) instead of
     through host numpy; it does not (cannot) make one song faster than one GPU's batch-1 speed,
     it removes the host round trip and frees the other ranks for other songs.
   * one song, faster (config 5, SURVEY 8e-iii): `CfgSplitPair` runs the conditional decoder pass

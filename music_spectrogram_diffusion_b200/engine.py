@@ -104,7 +104,7 @@ class Engine:
   def __init__(self, cfg: _native.MsdConfig, device: int = 0):
     self.lib = _native.load()
     if not torch.cuda.is_available():
-      raise _native.MsdError('no CUDA device: the sm_100a library cannot run (no CPU fallback)')
+      raise _native.MsdError('no CUDA device: the sm_90a library cannot run (no CPU fallback)')
     self.cfg = cfg
     self.device = torch.device('cuda', device)
     torch.cuda.set_device(self.device)

@@ -1,4 +1,4 @@
-"""Drop-in for `music_spectrogram_diffusion.inference` (msd/inference.py) on the B200 engine.
+"""Drop-in for `music_spectrogram_diffusion.inference` (msd/inference.py) on the CUDA engine.
 
 Keeps the reference's call surface:
   parse_training_gin_file(gin_file, gin_bindings) -> str          inference.py:32-65
@@ -154,7 +154,7 @@ def _build_from_gin(gin_config: str) -> Tuple[config.T5Config, config.DiffusionC
 
 
 class InferenceModel:
-  """Wrapper of the B200 engine with the reference's `InferenceModel` surface."""
+  """Wrapper of the CUDA engine with the reference's `InferenceModel` surface."""
 
   def __init__(self, checkpoint_path: str, gin_config: str, batch_size: int = 1,
                device: int = 0, rng: str = 'jax', precision: str = 'bf16'):

@@ -45,6 +45,34 @@ def test_reference_arm_runs_on_rank_zero_only():
   assert out.returncode == 0 and not [l for l in out.stdout.splitlines() if l.startswith('{')]
 
 
+def test_reference_arm_refuses_to_dump_outputs(tmp_path):
+  out = subprocess.run([sys.executable, os.path.join(ROOT, 'bench.py'), '--impl', 'reference',
+                        '--model', 'tiny', '--dump-outputs', str(tmp_path / 'd')],
+                       cwd=ROOT, capture_output=True, text=True, timeout=300)
+  assert out.returncode != 0 and '--dump-outputs' in out.stderr
+  assert not (tmp_path / 'd').exists()
+
+
+@pytest.mark.gpu
+def test_dump_outputs_is_float32_and_repeatable(tmp_path):
+  """--dump-outputs writes the last timed step's mel frames; same arguments, same bytes."""
+  import numpy as np
+  got = []
+  for name in ('a', 'b'):
+    out = subprocess.run([sys.executable, os.path.join(ROOT, 'bench.py'), '--model', 'tiny',
+                          '--segments', '2', '--steps', '2', '--warmup', '1', '--diffusion-steps', '8',
+                          '--no-song', '--no-cpu-baseline', '--no-traffic', '--no-timeline',
+                          '--dump-outputs', str(tmp_path / name)],
+                         cwd=ROOT, capture_output=True, text=True, timeout=600)
+    assert out.returncode == 0, out.stderr[-800:]
+    j = json.loads([l for l in out.stdout.splitlines() if l.startswith('{')][-1])
+    assert j['steps'] == 2
+    assert sorted(os.listdir(tmp_path / name)) == ['mel.npy']
+    got.append(np.load(tmp_path / name / 'mel.npy'))
+  assert got[0].dtype == np.float32 and got[0].shape == (2, 128, 128)
+  assert np.isfinite(got[0]).all() and np.array_equal(got[0], got[1])
+
+
 def test_flop_model_matches_the_survey_derivation():
   lengths = dict(config.TASK_FEATURE_LENGTHS_CONTEXT)
   per_step, once = bench.flops_model(config.t5_base(), lengths)

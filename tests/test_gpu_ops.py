@@ -1,4 +1,4 @@
-"""-m gpu: operator-level parity of the sm_100a kernels against the oracle's restatement of
+"""-m gpu: operator-level parity of the sm_90a kernels against the oracle's restatement of
 msd/layers.py (same shape of test as layers_test.py:375-387 / 285-330 / 450-484, at sizes the
 tensor-core kernels accept)."""
 import numpy as np
@@ -33,9 +33,9 @@ def test_dense_general(cuda_device, M, N, K, variant, block_n):
     (1, 2, 256, 2304, 5, True), (2, 2, 256, 768, 2, 'head'), (3, 2, 128, 256, 1, True),
     (8, 12, 256, 768, 0, False), (8, 12, 256, 2304, 0, True)])
 def test_dot_product_attention_tail_split(cuda_device, monkeypatch, nb, heads, Lq, Lk, tail, masked):
-  """128-key instance: long/short CTA pairs with the in-kernel merge (tail 0 = the automatic
-  choice, which is active for the 96-CTA grids of the last two cases); run twice to check the
-  hand-shake words re-arm."""
+  """128-key instance: long/short CTA pairs (the last `tail` key blocks go to a second CTA, merged
+  by the combine kernel; tail 0 = the automatic choice); run twice to check that a launch leaves
+  nothing behind."""
   from music_spectrogram_diffusion_b200 import engine
   monkeypatch.setenv('MSD_ATTN_BKV', '128')
   monkeypatch.setenv('MSD_ATTN_SPLITS', '1')
@@ -80,7 +80,7 @@ def _pack_gated_cols(b0, b1):
     (4096, 768, 768, 2304, 2048, 0, 0),      # self-attention projection -> QKV of the B = 8 step
     (4096, 768, 2048, 2048, 4096, 192, 256),  # wo -> next layer (explicit widths)
     (512, 768, 768, 768, 256, 64, 64),        # batch 1: 12 column tiles of partial row sums
-    (4096, 768, 768, 768, 4096, 64, 0),       # 192 tiles on 74 CTA pairs: several tiles per CTA
+    (4096, 768, 768, 768, 4096, 64, 0),       # 192 tiles of 64 columns: more CTAs than SMs
     (1280, 768, 512, 768, 600, 256, 0),       # 8 chunks per tile (ring refills), ragged split row
     (384, 512, 512, 1024, 128, 128, 0),       # odd number of 128-row blocks, other width
     (256, 256, 128, 256, 0, 256, 128)])       # one column tile, every row in the "hi" group
@@ -136,27 +136,24 @@ def test_deferred_normalisation_pair(cuda_device, M, d, K, N2, split_row, bn1, b
   assert rel < 1e-2, rel
 
 
-@pytest.mark.parametrize('bkv,merge', [(64, 1), (64, 0), (128, 1), (128, 0)])
+@pytest.mark.parametrize('bkv,draw', [(64, 1), (64, 0), (128, 1), (128, 0)])
 @pytest.mark.parametrize('splits', [0, 1, 3])
 @pytest.mark.parametrize('nb,heads,Lq,Lk,masked', [
     (1, 1, 128, 128, False), (2, 2, 128, 256, False), (2, 3, 256, 384, True),
     (1, 2, 256, 2304, True), (3, 2, 128, 128, True), (2, 2, 256, 768, True),
     (16, 12, 256, 256, False), (8, 12, 256, 2304, True)])
-def test_dot_product_attention(cuda_device, monkeypatch, nb, heads, Lq, Lk, masked, splits, bkv, merge):
-  """Both instances of the kernel (64-key blocks, two CTAs per SM; 128-key blocks, one CTA per
-  SM).  splits: 0 = automatic split-KV choice, 1 = single pass, 3 = forced 3-way split; merge:
-  partials merged by the owner CTA inside the kernel (1) or by the combine kernel (0).  The last
-  two shapes are the B = 8 decoder's self- and cross-attention.  Run twice: the merge flags re-arm."""
+def test_dot_product_attention(cuda_device, monkeypatch, nb, heads, Lq, Lk, masked, splits, bkv, draw):
+  """Both instances of the kernel (64-key and 128-key blocks).  splits: 0 = automatic split-KV
+  choice, 1 = single pass, 3 = forced 3-way split through the combine kernel; draw: two
+  independent random draws of the inputs and the mask.  The last two shapes are the B = 8 decoder's
+  self- and cross-attention.  Run twice: a launch leaves nothing behind in the workspace."""
   from music_spectrogram_diffusion_b200 import engine
   if splits == 3 and (Lk // bkv) % 3:
     pytest.skip('key blocks not divisible by 3')
-  if splits == 1 and merge == 0:
-    pytest.skip('same launch as merge=1')
   monkeypatch.setenv('MSD_ATTN_BKV', str(bkv))
-  monkeypatch.setenv('MSD_ATTN_MERGE', '0' if merge == 0 else ('2' if bkv == 128 else '1'))
   if splits:
     monkeypatch.setenv('MSD_ATTN_SPLITS', str(splits))
-  g = torch.Generator().manual_seed(nb * 1000 + Lk)
+  g = torch.Generator().manual_seed(nb * 1000 + Lk + 7 * (1 - draw))
   w = heads * 64
   q = bf16_round(torch.randn(nb, Lq, w, generator=g) * 0.5)
   k = bf16_round(torch.randn(nb, Lk, w, generator=g) * 0.5)

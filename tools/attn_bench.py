@@ -1,5 +1,5 @@
 """Attention micro-benchmark over the decoder's shapes (GPU): back-to-back launches, warm.
-Environment: MSD_ATTN_BKV / MSD_ATTN_SPLITS / MSD_ATTN_MERGE / MSD_ATTN_TAIL select the variant."""
+Environment: MSD_ATTN_BKV / MSD_ATTN_SPLITS / MSD_ATTN_TAIL select the variant."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

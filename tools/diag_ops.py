@@ -1,4 +1,4 @@
-"""GPU diagnostic (not a test): structured probes of the tcgen05 GEMM / attention kernels that
+"""GPU diagnostic (not a test): structured probes of the wgmma GEMM / attention kernels that
 make layout mistakes (swizzle, descriptor strides, major-ness) visible in the output."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

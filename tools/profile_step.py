@@ -1,5 +1,5 @@
 """Runs encode + a few uncaptured diffusion steps of the bench workload; meant to be wrapped in
-ncu (see profiles/README.md for the exact commands and launch indices)."""
+ncu."""
 import argparse, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
