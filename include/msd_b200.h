@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define MSD_B200_ABI_VERSION 5
+#define MSD_B200_ABI_VERSION 6
 
 typedef struct msd_ctx msd_ctx;
 
@@ -232,6 +232,33 @@ int msd_op_dense_deferred_norm(const float* a, const float* w_out, const float* 
 int msd_op_attention_f32(const float* q, const float* k, const float* v, const int32_t* key_mask,
                          int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, float* out,
                          void* stream);
+
+/* The attention kernel on caller-owned device buffers, launched the way the engine launches it
+ * (views into fused / cached buffers).  precision 0: bf16 q / k / v and the tensor-core kernel;
+ * 1: fp32 q / k / v and the fp32 kernel.
+ *   q / k / v   element offset + leading dimension (elements); head h reads columns h*64 .. +64 of
+ *               the view.  Q rows [nb * Lq]; K / V row of batch b, key j: b * kv_batch_rows +
+ *               kv_row0 + j (kv_batch_rows 0 = Lk).  k and v may be the same buffer.
+ *   key_mask    int32 [nb, mask_len] (> 0 = attend) or NULL; packed to mask_len / 32 words per row,
+ *               the attention reads words [mask_word0, mask_word0 + Lk / 32) of each row.
+ *   kv_static   bf16 mode: K / V and the mask are read ahead of the programmatic-dependency wait.
+ *               The hook completes all prior work on the stream, then rewrites the Q view (same
+ *               values) with a kernel of its own and launches the attention right behind it.
+ *   out         bf16; head h of row r written at out[o_col + r * o_ld + h*64 ..] (precision 0), or
+ *               as [hi | lo | hi] at out[o_col + r * 3 * o_ld + {0, o_ld, 2 o_ld} + h*64 ..]
+ *               (precision 1: o_ld is the width of one third).  Nothing else is written.
+ *   part_o / part_ml  split-KV workspace for up to 12 splits: f32 [nb * Lq * heads * 12 * 64] and
+ *               [nb * Lq * heads * 12 * 2].
+ *   splits      0 = automatic, else forced (<= 12); tail (bf16 only): > 0 moves the last `tail`
+ *               key blocks of an unsplit 128-key launch to a second CTA, 0 = none.
+ * The key-block size follows MSD_ATTN_BKV as in the engine.  Synchronises the stream. */
+int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq, const void* k,
+                          int64_t k_off, int32_t ldk, const void* v, int64_t v_off, int32_t ldv,
+                          int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32_t kv_batch_rows,
+                          int32_t kv_row0, const int32_t* key_mask, int32_t mask_len,
+                          int32_t mask_word0, int32_t kv_static, void* out, int64_t o_col,
+                          int32_t o_ld, float* part_o, float* part_ml, int32_t splits, int32_t tail,
+                          void* stream);
 
 /* LayerNorm (layers.py:632-649) followed by optional FiLM (layers.py:652-666) with explicit
  * scale|bias vector film [2*d] (NULL = none): out f32 (bf16-rounded) [rows, d]. */

@@ -136,8 +136,11 @@ SYMBOLS = [
     ('msd_op_dense_deferred_norm', ctypes.c_int,
      [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _I, _I, _P, _P, _P]),
     ('msd_op_attention_f32', ctypes.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
+    ('msd_op_attention_view', ctypes.c_int,
+     [_I, _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _I, _I, _I, _I, _I, _I,
+      _P, _I, _I, _I, _P, ctypes.c_int64, _I, _P, _P, _I, _I, _P]),
 ]
-ABI_VERSION = 5  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
+ABI_VERSION = 6  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
 
 _lib: Optional[ctypes.CDLL] = None
 

@@ -637,6 +637,18 @@ bf16_rows_to_f32_kernel(const bf16* s, int ld, int lo_off, float* d, long long r
   if (lo_off > 0) v += __bfloat162float(s[r * ld + lo_off + c]);
   d[i] = v;
 }
+// dst rows [rows, units] of 16-byte units with row strides in units; triggers its dependents at
+// entry, so a kernel launched behind it with PDL overlaps it up to its own dependency wait
+__global__ void __launch_bounds__(256)
+copy_rows_kernel(const uint4* s, long long lds, uint4* d, long long ldd, long long rows, int units) {
+  griddep_launch_dependents();
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  griddep_wait();
+  if (i >= rows * units) return;
+  const long long r = i / units;
+  const int c = static_cast<int>(i - r * units);
+  d[r * ldd + c] = s[r * lds + c];
+}
 __global__ void __launch_bounds__(256)
 mask_bits_kernel(const int* mask, long long words, uint32_t* bits) {
   const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
@@ -838,6 +850,18 @@ int launch_mask_bits(const int* mask, int nb, int L, uint32_t* bits, cudaStream_
   const long long words = static_cast<long long>(nb) * (L / 32);
   mask_bits_kernel<<<blocks_for(words * 32, 256), 256, 0, stream>>>(mask, words, bits);
   MSD_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+int launch_copy_rows(const void* src, long long ld_src, void* dst, long long ld_dst, long long rows,
+                     int row_bytes, cudaStream_t stream) {
+  MSD_REQUIRE(row_bytes % 16 == 0 && ld_src % 16 == 0 && ld_dst % 16 == 0 &&
+                  (reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0,
+              "copy_rows: rows, strides and pointers must be 16-byte aligned");
+  const int units = row_bytes / 16;
+  MSD_CUDA_CHECK(launch_kernel(copy_rows_kernel, dim3(blocks_for(rows * units, 256)), dim3(256), 0, stream,
+                               static_cast<const uint4*>(src), ld_src / 16, static_cast<uint4*>(dst),
+                               ld_dst / 16, rows, units));
+  ++g_launch_count;
   return 0;
 }
 

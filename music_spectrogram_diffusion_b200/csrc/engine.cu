@@ -869,7 +869,9 @@ static int decoder_layers_fused(msd_ctx* c, int nseg, int ncross, cudaStream_t s
     a.prep.split_row = split_row;
     a.prep.a = xn; a.prep.lda = d;
     a.prep.ss = ss; a.prep.ss_stride = ss_stride;
-    *parts = d / gemm_pick_wide_bn(M, d);
+    const int bn = gemm_resolve_block_n(a);   // the partial row sums are per column tile that runs
+    MSD_REQUIRE(bn > 0, "resid_prep: no tile width for M=%d d=%d", M, d);
+    *parts = d / bn;
     return launch_gemm(a, st);
   };
   auto row_scale = [&](GemmArgs& a, const float* lo, int parts_lo, const float* hi, int parts_hi,
@@ -1780,8 +1782,12 @@ int msd_op_dense_deferred_norm(const float* a, const float* w_out, const float* 
   bf16 *ab = nullptr, *wo = nullptr, *opnd = nullptr, *w2p = nullptr, *yb = nullptr;
   float* ss = nullptr;
   int* step0 = nullptr;
-  const int bn1 = block_n1 ? block_n1 : gemm_pick_wide_bn(M, d);
-  MSD_REQUIRE(bn1 > 0 && d % bn1 == 0, "msd_op_dense_deferred_norm: block_n1 must divide d");
+  GemmArgs g1;
+  memset(&g1, 0, sizeof(g1));
+  g1.M = M; g1.N = d; g1.K = K; g1.epilogue = EPI_RESID_PREP; g1.block_n = block_n1;
+  const int bn1 = gemm_resolve_block_n(g1);
+  MSD_REQUIRE(bn1 > 0, "msd_op_dense_deferred_norm: no valid tile width for d=%d (block_n1 %d)", d,
+              block_n1);
   const int parts = d / bn1;
   MSD_TRY(tb.get(&ab, static_cast<size_t>(M) * K));
   MSD_TRY(tb.get(&wo, static_cast<size_t>(d) * K));
@@ -1797,10 +1803,8 @@ int msd_op_dense_deferred_norm(const float* a, const float* w_out, const float* 
   else MSD_TRY(launch_pack_weight(w2, d, N2, w2p, d, 0, 0, 0, st));
   MSD_CUDA_CHECK(cudaMemcpyAsync(x_out, x, static_cast<size_t>(M) * d * sizeof(float),
                                  cudaMemcpyDeviceToDevice, st));
-  GemmArgs g1;
-  memset(&g1, 0, sizeof(g1));
-  g1.A = ab; g1.B = wo; g1.M = M; g1.N = d; g1.K = K; g1.lda = K; g1.ldb = K;
-  g1.epilogue = EPI_RESID_PREP; g1.out = x_out; g1.ldo = d; g1.resid = x_out; g1.block_n = bn1;
+  g1.A = ab; g1.B = wo; g1.lda = K; g1.ldb = K;
+  g1.out = x_out; g1.ldo = d; g1.resid = x_out; g1.block_n = bn1;
   g1.step = step0;
   g1.prep.g_lo = g_lo; g1.prep.g_hi = g_hi; g1.prep.split_row = split_row;
   g1.prep.a = opnd; g1.prep.lda = d; g1.prep.ss = ss; g1.prep.ss_stride = M;
@@ -1849,6 +1853,76 @@ int msd_op_attention_f32(const float* q, const float* k, const float* v, const i
   }
   MSD_TRY(launch_attention_f32(aa, st));
   MSD_TRY(launch_bf16_rows_to_f32(ob, 3 * w, w, out, static_cast<long long>(nb) * Lq, w, st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq, const void* k,
+                          int64_t k_off, int32_t ldk, const void* v, int64_t v_off, int32_t ldv,
+                          int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32_t kv_batch_rows,
+                          int32_t kv_row0, const int32_t* key_mask, int32_t mask_len,
+                          int32_t mask_word0, int32_t kv_static, void* out, int64_t o_col,
+                          int32_t o_ld, float* part_o, float* part_ml, int32_t splits, int32_t tail,
+                          void* stream) {
+  MSD_REQUIRE(q && k && v && out && part_o && part_ml, "msd_op_attention_view: null argument");
+  MSD_REQUIRE(precision == 0 || precision == 1, "msd_op_attention_view: precision must be 0 or 1");
+  MSD_REQUIRE(nb > 0 && heads > 0 && Lq > 0 && Lk > 0 && q_off >= 0 && k_off >= 0 && v_off >= 0 &&
+                  o_col >= 0 && kv_row0 >= 0 && kv_batch_rows >= 0,
+              "msd_op_attention_view: bad sizes or offsets");
+  MSD_REQUIRE(splits >= 0 && splits <= 12 && tail >= 0 && (precision == 0 || tail == 0),
+              "msd_op_attention_view: splits must be in [0, 12], tail >= 0 (bf16 mode only)");
+  MSD_REQUIRE(!key_mask || (mask_len % 128 == 0 && mask_word0 >= 0 && mask_word0 % 4 == 0 &&
+                            mask_word0 + Lk / 32 <= mask_len / 32),
+              "msd_op_attention_view: mask words [%d, %d) outside rows of %d keys", mask_word0,
+              mask_word0 + Lk / 32, mask_len);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t es = precision ? 4 : 2;
+  const int width = heads * 64;
+  const long long rows_q = static_cast<long long>(nb) * Lq;
+  char* qv = static_cast<char*>(q) + q_off * es;
+  TempBufs tb;
+  uint32_t* bits = nullptr;
+  if (key_mask) {
+    MSD_TRY(tb.get(&bits, static_cast<size_t>(nb) * (mask_len / 32)));
+    MSD_TRY(launch_mask_bits(key_mask, nb, mask_len, bits, st));
+  }
+  // K, V and the mask must be complete before the attention starts (kv_static reads them ahead of
+  // its dependency wait, as after the plain first launch of a diffusion step).  Q is then written
+  // back from a staging copy by a kernel of its own, so that the attention is a PDL launch behind a
+  // live predecessor, as in the step graph.
+  char* stage = nullptr;
+  MSD_TRY(tb.get(&stage, static_cast<size_t>(rows_q) * width * es));
+  MSD_CUDA_CHECK(cudaMemcpy2DAsync(stage, width * es, qv, ldq * es, width * es, rows_q,
+                                   cudaMemcpyDeviceToDevice, st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  MSD_TRY(launch_copy_rows(stage, static_cast<long long>(width * es), qv, static_cast<long long>(ldq) * es,
+                           rows_q, static_cast<int>(width * es), st));
+  const uint32_t* mbits = bits ? bits + mask_word0 : nullptr;
+  if (precision == 0) {
+    AttnArgs a;
+    memset(&a, 0, sizeof(a));
+    a.Q = reinterpret_cast<const bf16*>(qv); a.ldq = ldq;
+    a.K = static_cast<const bf16*>(k) + k_off; a.ldk = ldk;
+    a.V = static_cast<const bf16*>(v) + v_off; a.ldv = ldv;
+    a.O = static_cast<bf16*>(out) + o_col; a.ldo = o_ld;
+    a.nbatch = nb; a.heads = heads; a.Lq = Lq; a.Lk = Lk;
+    a.mask_bits = mbits; a.mask_stride_words = mask_len / 32;
+    a.part_o = part_o; a.part_ml = part_ml; a.splits = splits; a.max_splits = 12; a.tail = tail;
+    a.kv_static = kv_static; a.kv_batch_rows = kv_batch_rows; a.kv_row0 = kv_row0;
+    MSD_TRY(launch_attention(a, st));
+  } else {
+    AttnF32Args a;
+    memset(&a, 0, sizeof(a));
+    a.Q = reinterpret_cast<const float*>(qv); a.ldq = ldq;
+    a.K = static_cast<const float*>(k) + k_off; a.ldk = ldk;
+    a.V = static_cast<const float*>(v) + v_off; a.ldv = ldv;
+    a.O = static_cast<bf16*>(out) + o_col; a.o_third = o_ld;
+    a.nbatch = nb; a.heads = heads; a.Lq = Lq; a.Lk = Lk;
+    a.mask_bits = mbits; a.mask_stride_words = mask_len / 32;
+    a.kv_batch_rows = kv_batch_rows; a.kv_row0 = kv_row0;
+    a.part_o = part_o; a.part_ml = part_ml; a.splits = splits; a.max_splits = 12;
+    MSD_TRY(launch_attention_f32(a, st));
+  }
   MSD_CUDA_CHECK(cudaStreamSynchronize(st));
   return 0;
 }

@@ -374,23 +374,32 @@ int gemm_pick_block_n(int M, int N) {
   return 0;
 }
 
+static bool gemm_wide_variant(const GemmArgs& a) {
+  static const int forced_variant = [] {
+    const char* e = getenv("MSD_GEMM_VARIANT");  // debugging aid: 1 forces variant 1's tile choice
+    return e ? atoi(e) : 0;
+  }();
+  return (forced_variant ? forced_variant : a.variant) != 1;
+}
+
+int gemm_resolve_block_n(const GemmArgs& a) {
+  const bool wide = gemm_wide_variant(a);
+  const int bn = a.block_n ? a.block_n
+                           : (wide ? gemm_pick_wide_bn(a.M, a.N) : gemm_pick_block_n(a.M, a.N));
+  const bool allowed = bn == 64 || bn == 128 || bn == 256 || (wide && bn == 192) ||
+                       (wide && bn == 96 && !epi_is_bf16_out(a.epilogue));
+  return allowed && a.N % bn == 0 ? bn : 0;
+}
+
 int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   static int configured = gemm_configure();
   if (configured != 0) return configured;
   MSD_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "gemm: empty problem M=%d N=%d K=%d", a.M, a.N, a.K);
   MSD_REQUIRE(a.K % BLOCK_K == 0, "gemm: K=%d must be a multiple of %d", a.K, BLOCK_K);
   MSD_REQUIRE(a.M % BLOCK_M == 0, "gemm: M=%d must be a multiple of %d", a.M, BLOCK_M);
-  static const int forced_variant = [] {
-    const char* e = getenv("MSD_GEMM_VARIANT");  // debugging aid: 1 forces variant 1's tile choice
-    return e ? atoi(e) : 0;
-  }();
-  const bool wide = (forced_variant ? forced_variant : a.variant) != 1;
-  int bn = a.block_n ? a.block_n
-                     : (wide ? gemm_pick_wide_bn(a.M, a.N) : gemm_pick_block_n(a.M, a.N));
-  MSD_REQUIRE(bn == 64 || bn == 128 || bn == 256 || (wide && bn == 192) ||
-                  (wide && bn == 96 && !epi_is_bf16_out(a.epilogue)),
-              "gemm: N=%d has no valid tile width (block_n %d)", a.N, bn);
-  MSD_REQUIRE(a.N % bn == 0, "gemm: N=%d not a multiple of block_n=%d", a.N, bn);
+  const int bn = gemm_resolve_block_n(a);
+  MSD_REQUIRE(bn != 0, "gemm: N=%d has no valid tile width (block_n %d, variant %d)", a.N, a.block_n,
+              gemm_wide_variant(a) ? 0 : 1);
   MSD_REQUIRE(a.ldo % 8 == 0, "gemm: ldo=%d must be a multiple of 8", a.ldo);
 
   CUtensorMap ta, tb;

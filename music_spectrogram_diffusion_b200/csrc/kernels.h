@@ -145,6 +145,10 @@ int gemm_configure();  // opt in to the kernels' dynamic shared memory sizes (id
 // Box rows the A / B maps must be built with for a given block_n choice.
 int gemm_pick_block_n(int M, int N);
 int gemm_pick_wide_bn(int M, int N);
+// The tile width launch_gemm(a) runs with (a.block_n, a.variant, MSD_GEMM_VARIANT and the shape),
+// or 0 when that width is not allowed.  Whoever sizes per-tile outputs (EPI_RESID_PREP's partial
+// row sums: N / width of them) must take the width from here.
+int gemm_resolve_block_n(const GemmArgs& a);
 
 // ---------------------------------------------------------------------------
 // Attention: O = softmax(Q K^T + keymask) V, no 1/sqrt(d), head_dim 64.
@@ -320,6 +324,10 @@ int launch_sgemm_f32(const float* A, const float* B, float* C, int ldc, int M, i
 int launch_f32_to_bf16(const float* src, bf16* dst, long long n, cudaStream_t stream);
 int launch_bf16_to_f32(const bf16* src, float* dst, long long n, cudaStream_t stream);
 int launch_mask_bits(const int* mask, int nb, int L, uint32_t* bits, cudaStream_t stream);
+// dst[r * ld_dst + c] = src[r * ld_src + c] for `rows` rows of row_bytes bytes (strides in bytes,
+// everything 16-byte aligned); a PDL launch that lets its dependents start at once
+int launch_copy_rows(const void* src, long long ld_src, void* dst, long long ld_dst, long long rows,
+                     int row_bytes, cudaStream_t stream);
 // dst [rows, cols] f32 = src[r * ld + c] (+ src[r * ld + lo_off + c] when lo_off > 0)
 int launch_bf16_rows_to_f32(const bf16* src, int ld, int lo_off, float* dst, long long rows, int cols,
                             cudaStream_t stream);

@@ -310,6 +310,92 @@ def op_attention_f32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor,
   return out
 
 
+ATTN_MAX_SPLITS = 12   # split-KV workspace of msd_op_attention_view, in splits
+
+
+def attention_workspace(nb: int, lq: int, heads: int, device: torch.device):
+  """(part_o, part_ml) f32 buffers for op_attention_view with up to ATTN_MAX_SPLITS splits."""
+  rows = nb * lq * heads * ATTN_MAX_SPLITS
+  return (torch.empty(rows * 64, dtype=torch.float32, device=device),
+          torch.empty(rows * 2, dtype=torch.float32, device=device))
+
+
+def _check_view(name: str, t: torch.Tensor, off: int, ld: int, rows: int, cols: int, elem: int) -> None:
+  """The view (rows x cols from element `off`, row stride `ld`) lies inside t, no row wraps."""
+  if not t.is_contiguous():
+    raise ValueError(f'{name}: tensor must be contiguous')
+  align = 16 // elem
+  if off < 0 or ld <= 0 or off % align or ld % align:
+    raise ValueError(f'{name}: offset {off} / leading dimension {ld} must be non-negative multiples '
+                     f'of {align} elements')
+  row0, col0 = divmod(off, ld)
+  if col0 + cols > ld:
+    raise ValueError(f'{name}: columns [{col0}, {col0 + cols}) exceed the leading dimension {ld}')
+  if (row0 + rows) * ld > t.numel():
+    raise ValueError(f'{name}: rows [{row0}, {row0 + rows}) of {ld} elements exceed the '
+                     f'{t.numel()} elements of the tensor')
+
+
+def op_attention_view(q: torch.Tensor, q_off: int, ldq: int, k: torch.Tensor, k_off: int, ldk: int,
+                      v: torch.Tensor, v_off: int, ldv: int, nb: int, heads: int, lq: int, lk: int,
+                      out: torch.Tensor, o_col: int, o_ld: int, part_o: torch.Tensor,
+                      part_ml: torch.Tensor, key_mask: Optional[torch.Tensor] = None,
+                      mask_word0: int = 0, kv_batch_rows: int = 0, kv_row0: int = 0,
+                      kv_static: int = 0, splits: int = 0, tail: int = 0,
+                      precision: str = 'bf16') -> None:
+  """The attention kernel over views of caller-owned device buffers (msd_op_attention_view):
+  q / k / v are bf16 (precision 'bf16') or f32 ('fp32_accurate') tensors addressed by element
+  offset + leading dimension, out is bf16 and is written in place (fp32_accurate: [hi | lo | hi]
+  with o_ld the width of one third), key_mask int32 [nb, mask_len].  Every view is checked to lie
+  inside its tensor before the library is called."""
+  if precision not in PRECISIONS:
+    raise ValueError(f'unknown precision {precision!r}')
+  acc = PRECISIONS[precision]
+  dt, elem = (torch.float32, 4) if acc else (torch.bfloat16, 2)
+  width = heads * 64
+  if nb <= 0 or heads <= 0 or lq <= 0 or lk <= 0 or lq % 128 or lk % 128:
+    raise ValueError(f'nb={nb}, heads={heads}: Lq={lq} and Lk={lk} must be positive multiples of 128')
+  for name, t in (('q', q), ('k', k), ('v', v)):
+    if t.dtype != dt or not t.is_cuda:
+      raise ValueError(f'{name}: expected a {dt} CUDA tensor, got {t.dtype} on {t.device}')
+  if out.dtype != torch.bfloat16 or not out.is_cuda:
+    raise ValueError('out: expected a bf16 CUDA tensor')
+  kbr = kv_batch_rows if kv_batch_rows > 0 else lk
+  if kv_batch_rows < 0 or kv_row0 < 0 or kv_row0 + lk > kbr:
+    raise ValueError(f'key rows [{kv_row0}, {kv_row0 + lk}) exceed the {kbr} rows per batch')
+  _check_view('q', q, q_off, ldq, nb * lq, width, elem)
+  _check_view('k', k, k_off, ldk, nb * kbr, width, elem)
+  _check_view('v', v, v_off, ldv, nb * kbr, width, elem)
+  if acc:
+    if o_col + width > o_ld:
+      raise ValueError(f'out: columns [{o_col}, {o_col + width}) exceed the third of width {o_ld}')
+    _check_view('out', out, o_col, 3 * o_ld, nb * lq, 2 * o_ld + width, 2)
+  else:
+    _check_view('out', out, o_col, o_ld, nb * lq, width, 2)
+  mask_len = 0
+  if key_mask is not None:
+    if key_mask.dtype != torch.int32 or not key_mask.is_contiguous() or key_mask.dim() != 2 \
+        or key_mask.shape[0] != nb:
+      raise ValueError(f'key_mask: expected contiguous int32 [{nb}, mask_len]')
+    mask_len = key_mask.shape[1]
+    if mask_len % 128 or mask_word0 < 0 or mask_word0 % 4 or mask_word0 + lk // 32 > mask_len // 32:
+      raise ValueError(f'key_mask: words [{mask_word0}, {mask_word0 + lk // 32}) outside rows of '
+                       f'{mask_len // 32} words (mask_len and the start word: multiples of 128 / 4)')
+  elif mask_word0:
+    raise ValueError('mask_word0 without a key_mask')
+  need = nb * lq * heads * ATTN_MAX_SPLITS
+  for name, t, n in (('part_o', part_o, need * 64), ('part_ml', part_ml, need * 2)):
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() < n:
+      raise ValueError(f'{name}: expected a contiguous f32 tensor of at least {n} elements')
+  if not 0 <= splits <= ATTN_MAX_SPLITS or tail < 0 or (acc and tail):
+    raise ValueError(f'splits={splits} must be in [0, {ATTN_MAX_SPLITS}]; tail={tail} >= 0 (bf16 only)')
+  lib = _native.load()
+  _native.check(lib.msd_op_attention_view(
+      acc, _ptr(q), q_off, ldq, _ptr(k), k_off, ldk, _ptr(v), v_off, ldv, nb, heads, lq, lk,
+      kv_batch_rows, kv_row0, _ptr(key_mask), mask_len, mask_word0, int(kv_static), _ptr(out), o_col,
+      o_ld, _ptr(part_o), _ptr(part_ml), splits, tail, _stream(q.device)), 'msd_op_attention_view')
+
+
 def op_jax_bits(seed: int, step: int, n: int, device: torch.device) -> torch.Tensor:
   """Raw uint32 words of the device jax.random stream (as int32 storage; view as uint32)."""
   out = torch.empty(n, dtype=torch.int32, device=device)

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from oracle import msd_oracle as O
+from tests import test_gpu_attention_views as AV
 from tests.helpers import bf16_round
 
 pytestmark = pytest.mark.gpu
@@ -46,7 +47,6 @@ def test_dot_product_attention_tail_split(cuda_device, monkeypatch, nb, heads, L
   k = bf16_round(torch.randn(nb, Lk, w, generator=g) * 0.5)
   v = bf16_round(torch.randn(nb, Lk, w, generator=g))
   mask = None
-  bias = None
   if masked:
     mask = (torch.rand(nb, Lk, generator=g) > 0.3).to(torch.int32)
     if masked == 'head':
@@ -55,18 +55,12 @@ def test_dot_product_attention_tail_split(cuda_device, monkeypatch, nb, heads, L
       mask[0, Lk // 2:] = 0                    # the short CTA of batch 0 has nothing to attend to
     if nb > 2:
       mask[2, :] = 0                           # neither has -> zeros
-    qm = torch.ones(nb, Lq)
-    m4 = O.make_attention_mask(qm, mask.float())
-    bias = torch.where(m4 > 0, torch.zeros_like(m4), torch.full_like(m4, -1e10))
-  want = O.dot_product_attention(q.view(nb, Lq, heads, 64), k.view(nb, Lk, heads, 64),
-                                 v.view(nb, Lk, heads, 64), bias).reshape(nb, Lq, w)
-  if masked:
-    want = O.zero_activations_if_masked(want, m4)
-  for _ in range(2):
-    got = engine.op_attention(q.to(cuda_device), k.to(cuda_device), v.to(cuda_device),
-                              None if mask is None else mask.to(cuda_device), heads).cpu()
-    err = (got - want).abs().max().item()
-    assert err < 3e-2, f'max err {err}'
+  q, k, v = q.to(cuda_device), k.to(cuda_device), v.to(cuda_device)
+  mask = None if mask is None else mask.to(cuda_device)
+  want, wabs = AV.reference(q, k, v, mask)
+  for run in range(2):
+    got = engine.op_attention(q, k, v, mask, heads)
+    AV.check_rounding_bound(got, want, wabs, f'nb={nb} Lk={Lk} tail={tail} masked={masked} run {run}')
 
 
 def _pack_gated_cols(b0, b1):
@@ -159,25 +153,18 @@ def test_dot_product_attention(cuda_device, monkeypatch, nb, heads, Lq, Lk, mask
   k = bf16_round(torch.randn(nb, Lk, w, generator=g) * 0.5)
   v = bf16_round(torch.randn(nb, Lk, w, generator=g))
   mask = None
-  bias = None
   if masked:
     mask = (torch.rand(nb, Lk, generator=g) > 0.3).to(torch.int32)
     mask[0, Lk // 2:] = 0                      # a run of fully masked key blocks
     if nb > 2:
       mask[2, :] = 0                           # a row with nothing to attend to -> zeros
-    qm = torch.ones(nb, Lq)
-    m4 = O.make_attention_mask(qm, mask.float())
-    bias = torch.where(m4 > 0, torch.zeros_like(m4), torch.full_like(m4, -1e10))
-  want = O.dot_product_attention(q.view(nb, Lq, heads, 64), k.view(nb, Lk, heads, 64),
-                                 v.view(nb, Lk, heads, 64), bias).reshape(nb, Lq, w)
-  if masked:
-    want = O.zero_activations_if_masked(want, m4)
-  for _ in range(2):
-    got = engine.op_attention(q.to(cuda_device), k.to(cuda_device), v.to(cuda_device),
-                              None if mask is None else mask.to(cuda_device), heads).cpu()
-    err = (got - want).abs().max().item()
-    assert torch.isfinite(got).all()
-    assert err < 3e-2, f'max err {err}'
+  q, k, v = q.to(cuda_device), k.to(cuda_device), v.to(cuda_device)
+  mask = None if mask is None else mask.to(cuda_device)
+  want, wabs = AV.reference(q, k, v, mask)
+  for run in range(2):
+    got = engine.op_attention(q, k, v, mask, heads)
+    AV.check_rounding_bound(got, want, wabs,
+                            f'nb={nb} Lk={Lk} splits={splits} bkv={bkv} draw={draw} run {run}')
 
 
 @pytest.mark.parametrize('rows,d,film', [(128, 128, False), (256, 768, True), (100, 512, True)])

@@ -142,7 +142,7 @@ def test_c_abi_exports_every_declared_symbol(native_lib):
   assert declared == bound, (declared ^ bound)
   for name in declared:
     assert hasattr(native_lib, name), name
-  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 5
+  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 6
   assert isinstance(native_lib.msd_last_error(), bytes)
 
 
