@@ -117,6 +117,16 @@ int msd_encode(msd_ctx* ctx, const int32_t* tokens, const float* ctx_features,
 int msd_sample(msd_ctx* ctx, const float* init_z, const float* noise, uint64_t seed,
                float* mel_out, void* stream);
 
+/* As msd_sample with generated noise, but row b of the batch of the preceding msd_encode draws
+ * init_z and every step's noise from seeds[b] alone (host array of cur_batch entries): exactly
+ * the draws msd_sample(seeds[b]) makes at batch 1.  This lets several songs share one batch
+ * (one song per row, beam/evaluation.py:156-223 runs each song on its own with predict(batch),
+ * inference.py:203) without a song's audio depending on which other songs share its batch or
+ * which row it sits in.  The same captured step graph serves msd_sample; rng_kind selects the
+ * stream as there.  Refused (-1) without a preceding msd_encode or with a peer attached
+ * (msd_p2p_attach). */
+int msd_sample_rows(msd_ctx* ctx, const uint64_t* seeds, float* mel_out, void* stream);
+
 /* ---- one song on two GPUs: classifier-free guidance split (BASELINE config 5, SURVEY 8e-iii) ----
  * The two decoder passes of a reverse step (diffusion_utils.py:415, 428-429) are independent until
  * the guidance combine (430-433).  With a peer attached, a context runs ONE of them (role 1: the

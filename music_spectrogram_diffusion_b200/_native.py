@@ -116,6 +116,7 @@ SYMBOLS = [
     ('msd_load_weights', ctypes.c_int, [_P, ctypes.POINTER(MsdTensor), _I]),
     ('msd_encode', ctypes.c_int, [_P, _P, _P, _P, _I, _P]),
     ('msd_sample', ctypes.c_int, [_P, _P, _P, ctypes.c_uint64, _P, _P]),
+    ('msd_sample_rows', ctypes.c_int, [_P, _P, _P, _P]),
     ('msd_p2p_export', ctypes.c_int, [_P, _P]),
     ('msd_p2p_attach', ctypes.c_int, [_P, _P, _I]),
     ('msd_p2p_detach', ctypes.c_int, [_P]),

@@ -280,6 +280,7 @@ __device__ __forceinline__ float4 jax_normal4(const uint32_t* key, long long n, 
 __device__ __forceinline__ void sampler_step_body(const SamplerArgs& a, int step,
                                                   const float* noise_base, float* mel_base,
                                                   unsigned long long seed, long long i4,
+                                                  bool per_row,
                                                   const float* eps_cond = nullptr,
                                                   const float* eps_uncond = nullptr) {
   const long long idx = i4 * 4;
@@ -343,10 +344,19 @@ __device__ __forceinline__ void sampler_step_body(const SamplerArgs& a, int step
       if (noise_base != nullptr) {
         nz = *reinterpret_cast<const float4*>(noise_base + static_cast<size_t>(step) * a.n + idx);
       } else {
+        long long n = a.n, j4 = i4;
+        const uint32_t* keys = a.rng_keys;
+        if (per_row) {  // row b's own draw of n_row elements (i4 < 2^30: n < 2^32 is required)
+          const unsigned int b = static_cast<unsigned int>(i4) / static_cast<unsigned int>(a.n_row >> 2);
+          n = a.n_row;
+          j4 = i4 - static_cast<long long>(b) * (a.n_row >> 2);
+          keys = a.row_keys + b * a.row_key_stride;
+          if (a.rng_kind == 0) seed = a.row_seeds[b];
+        }
         nz = a.rng_kind == 1
-                 ? jax_normal4(a.rng_keys + 2 * (step + 1), a.n, i4)
+                 ? jax_normal4(keys + 2 * (step + 1), n, j4)
                  : philox_normal4(seed, static_cast<uint32_t>(step) + 1u,
-                                  static_cast<unsigned long long>(i4));
+                                  static_cast<unsigned long long>(j4));
       }
     }
     zn.x = c_z * z.x + c_x0 * x0.x + sigma * nz.x; zn.y = c_z * z.y + c_x0 * x0.y + sigma * nz.y;
@@ -387,7 +397,7 @@ __global__ void __launch_bounds__(256) sampler_step_kernel(const SamplerArgs a) 
   if (a.run == nullptr) {
     const int step = *a.step;
     prefetch_next_film(a, step, i4);
-    if (i4 * 4 < a.n) sampler_step_body(a, step, a.noise, a.mel_out, a.seed, i4);
+    if (i4 * 4 < a.n) sampler_step_body(a, step, a.noise, a.mel_out, a.seed, i4, false);
     return;
   }
   // Per-call arguments and the step index live in device memory (RunArgs).  The step advance is
@@ -412,6 +422,7 @@ __global__ void __launch_bounds__(256) sampler_step_kernel(const SamplerArgs a) 
   const float* noise_base = a.run->noise;
   float* mel_base = a.run->mel_out;
   const unsigned long long seed = a.run->seed;
+  const bool per_row = a.run->per_row != 0;
   if (a.xrole != 0) {
     // ---- guidance split: send my pass's eps to the peer, receive the peer's
     __shared__ unsigned int s_seq;
@@ -447,22 +458,34 @@ __global__ void __launch_bounds__(256) sampler_step_kernel(const SamplerArgs a) 
     const float* other = a.xlocal + par;
     const float* ec = a.xrole == 1 ? a.eps : other;
     const float* eu = a.xrole == 1 ? other : a.eps;
-    if (i4 * 4 < a.n) sampler_step_body(a, step, noise_base, mel_base, seed, i4, ec, eu);
+    if (i4 * 4 < a.n) sampler_step_body(a, step, noise_base, mel_base, seed, i4, per_row, ec, eu);
     return;
   }
-  if (i4 * 4 < a.n) sampler_step_body(a, step, noise_base, mel_base, seed, i4);
+  if (i4 * 4 < a.n) sampler_step_body(a, step, noise_base, mel_base, seed, i4, per_row);
 }
 
 __global__ void __launch_bounds__(256)
 init_z_kernel(const float* init_z, float* z, bf16* zs, long long n, int n_dims,
-              unsigned long long seed, int rng_kind, const uint32_t* rng_keys) {
+              unsigned long long seed, int rng_kind, const uint32_t* rng_keys, long long n_row,
+              long long row_key_stride, const unsigned long long* row_seeds) {
   const long long i4 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long idx = i4 * 4;
   if (idx >= n) return;
   float4 v;
-  if (init_z != nullptr) v = *reinterpret_cast<const float4*>(init_z + idx);
-  else if (rng_kind == 1) v = jax_normal4(rng_keys, n, i4);
-  else v = philox_normal4(seed, 0u, static_cast<unsigned long long>(i4));
+  if (init_z != nullptr) {
+    v = *reinterpret_cast<const float4*>(init_z + idx);
+  } else {
+    long long m = n, j4 = i4;
+    if (n_row > 0) {  // per-row streams, as in sampler_step_body
+      const unsigned int b = static_cast<unsigned int>(i4) / static_cast<unsigned int>(n_row >> 2);
+      m = n_row;
+      j4 = i4 - static_cast<long long>(b) * (n_row >> 2);
+      rng_keys += b * row_key_stride;
+      if (rng_kind == 0) seed = row_seeds[b];
+    }
+    v = rng_kind == 1 ? jax_normal4(rng_keys, m, j4)
+                      : philox_normal4(seed, 0u, static_cast<unsigned long long>(j4));
+  }
   *reinterpret_cast<float4*>(z + idx) = v;
   store_split4(zs, idx, n_dims, v);
 }
@@ -762,11 +785,16 @@ int launch_jax_normal(uint32_t k0, uint32_t k1, long long n, float* out, cudaStr
 
 int launch_init_z(const float* init_z, float* z, bf16* z_split, long long n, int n_dims,
                   unsigned long long seed, cudaStream_t stream, int rng_kind,
-                  const uint32_t* rng_keys) {
+                  const uint32_t* rng_keys, long long n_row, long long row_key_stride,
+                  const unsigned long long* row_seeds) {
   MSD_REQUIRE(rng_kind == 0 || (rng_keys != nullptr && n % 8 == 0 && n < (1ll << 32)),
               "init_z: the jax stream needs its key table and a draw of k*8 < 2^32 elements");
+  MSD_REQUIRE(n_row == 0 || (n_row > 0 && n_row % 8 == 0 && n % n_row == 0 && n < (1ll << 32) &&
+                             rng_keys != nullptr && row_seeds != nullptr),
+              "init_z: per-row streams need rows of k*8 elements, n < 2^32 and both row tables");
   init_z_kernel<<<blocks_for(n / 4, 256), 256, 0, stream>>>(init_z, z, z_split, n, n_dims, seed,
-                                                            rng_kind, rng_keys);
+                                                            rng_kind, rng_keys, n_row,
+                                                            row_key_stride, row_seeds);
   MSD_CUDA_CHECK(cudaGetLastError());
   ++g_launch_count;
   return 0;

@@ -203,6 +203,12 @@ struct msd_ctx {
   float* coef = nullptr;      // [steps, MSD_STEP_COLS] device
   uint32_t* rng_keys = nullptr;  // [steps + 1, 2] jax.random keys of the current seed (rng_kind 1)
   unsigned long long rng_keys_seed = ~0ull;
+  // per-row noise streams (msd_sample_rows): jax keys [Bmax][steps + 1][2] and Philox seeds [Bmax]
+  // of each batch row's own seed, device; host copies of the seeds they were built from
+  uint32_t* row_keys = nullptr;
+  unsigned long long* row_seeds = nullptr;
+  std::vector<unsigned long long> row_seeds_host;
+  std::vector<char> row_keys_valid;
   std::vector<float> coef_host;
 
   // ---- activations (decoder, rows = passes*B*N)
@@ -996,6 +1002,9 @@ static int sampler_step(msd_ctx* c, int B, const float* noise, unsigned long lon
   a.n_dims = c->nd; a.passes = c->passes; a.cond_weight = c->cfg.eval_condition_weight;
   a.clip_x0 = c->cfg.clip_x0; a.ddim = c->cfg.sampler == 1; a.feat_min = c->cfg.feature_min; a.feat_max = c->cfg.feature_max;
   a.seed = seed; a.rng_kind = c->cfg.rng_kind; a.rng_keys = c->rng_keys;
+  a.n_row = static_cast<long long>(c->N) * c->nd;
+  a.row_keys = c->row_keys; a.row_key_stride = 2 * (static_cast<long long>(c->cfg.num_steps) + 1);
+  a.row_seeds = c->row_seeds;
   a.run = use_run ? c->run : nullptr;
   a.film = c->film;
   a.film_step_floats = static_cast<long long>(2) * c->cfg.num_decoder_layers * 2 * c->d;
@@ -1188,6 +1197,10 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
       rc = -2;
       break;
     }
+    if ((rc = A.alloc(&c->row_keys, static_cast<size_t>(c->Bmax) * (cfg->num_steps + 1) * 2))) break;
+    if ((rc = A.alloc(&c->row_seeds, static_cast<size_t>(c->Bmax)))) break;
+    c->row_seeds_host.assign(c->Bmax, 0ull);
+    c->row_keys_valid.assign(c->Bmax, 0);
     build_step_table(*cfg, c->coef_host);
     if (cudaMemcpy(c->coef, c->coef_host.data(), c->coef_host.size() * sizeof(float),
                    cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -1345,33 +1358,17 @@ int msd_decode_eps(msd_ctx* c, const float* z, int32_t step_i, int32_t condition
   return 0;
 }
 
-int msd_sample(msd_ctx* c, const float* init_z, const float* noise, uint64_t seed, float* mel_out,
-               void* stream) {
-  MSD_REQUIRE(c && mel_out, "msd_sample: null argument");
-  MSD_REQUIRE(c->cur_batch > 0, "msd_sample: call msd_encode first");
-  cudaStream_t caller = reinterpret_cast<cudaStream_t>(stream);
-  MSD_TRY(begin_on(c, caller));
-  cudaStream_t st = c->work;
+// The reverse steps of msd_sample / msd_sample_rows after init_z: per-call arguments to c->run,
+// then num_steps launches of the step graph (captured on first use for this batch size).
+static int run_steps(msd_ctx* c, const float* noise, unsigned long long seed, int per_row,
+                     float* mel_out, cudaStream_t st) {
   const int B = c->cur_batch, steps = c->cfg.num_steps;
-  const long long n = static_cast<long long>(B) * c->N * c->nd;
-  if (c->cfg.rng_kind == 1 && c->rng_keys_seed != seed) {
-    // PRNGKey(seed) and fold_in(key, i) for every scan index (host threefry, 8 KB upload); the
-    // captured step graph reads the table, so a new seed does not force a re-capture
-    std::vector<uint32_t> keys(2 * (static_cast<size_t>(steps) + 1));
-    keys[0] = static_cast<uint32_t>(seed >> 32);
-    keys[1] = static_cast<uint32_t>(seed);
-    for (int i = 0; i < steps; ++i)
-      threefry2x32_host(keys[0], keys[1], 0u, static_cast<uint32_t>(i), &keys[2 * (i + 1)]);
-    MSD_CUDA_CHECK(cudaMemcpyAsync(c->rng_keys, keys.data(), keys.size() * sizeof(uint32_t),
-                                   cudaMemcpyHostToDevice, st));
-    MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-    c->rng_keys_seed = seed;
-  }
-  MSD_TRY(launch_init_z(init_z, c->z, c->z_split, n, c->nd, seed, st, c->cfg.rng_kind, c->rng_keys));
   // Per-call arguments + the step index go to device memory: the captured graph reads them from
-  // there, so neither a new noise tensor / output buffer / seed nor the step forces a re-capture.
+  // there, so neither a new noise tensor / output buffer / seed / noise mode nor the step forces a
+  // re-capture.
   RunArgs ra;
   ra.noise = noise; ra.mel_out = mel_out; ra.seed = seed; ra.step = steps - 1; ra.done = 0u;
+  ra.per_row = per_row;
   // guidance split: exchange sequence numbers 1, 2, ... identical on both ranks (they make the same
   // calls), parity = buffer half
   ra.xseq = static_cast<unsigned int>(c->xcalls * static_cast<unsigned long long>(steps) + 1ull);
@@ -1406,6 +1403,79 @@ int msd_sample(msd_ctx* c, const float* init_z, const float* noise, uint64_t see
     MSD_CUDA_CHECK(cudaGraphLaunch(c->graph_exec, st));
     g_launch_count += c->graph_nodes;
   }
+  return 0;
+}
+
+int msd_sample(msd_ctx* c, const float* init_z, const float* noise, uint64_t seed, float* mel_out,
+               void* stream) {
+  MSD_REQUIRE(c && mel_out, "msd_sample: null argument");
+  MSD_REQUIRE(c->cur_batch > 0, "msd_sample: call msd_encode first");
+  cudaStream_t caller = reinterpret_cast<cudaStream_t>(stream);
+  MSD_TRY(begin_on(c, caller));
+  cudaStream_t st = c->work;
+  const int B = c->cur_batch, steps = c->cfg.num_steps;
+  const long long n = static_cast<long long>(B) * c->N * c->nd;
+  if (c->cfg.rng_kind == 1 && c->rng_keys_seed != seed) {
+    // PRNGKey(seed) and fold_in(key, i) for every scan index (host threefry, 8 KB upload); the
+    // captured step graph reads the table, so a new seed does not force a re-capture
+    std::vector<uint32_t> keys(2 * (static_cast<size_t>(steps) + 1));
+    keys[0] = static_cast<uint32_t>(seed >> 32);
+    keys[1] = static_cast<uint32_t>(seed);
+    for (int i = 0; i < steps; ++i)
+      threefry2x32_host(keys[0], keys[1], 0u, static_cast<uint32_t>(i), &keys[2 * (i + 1)]);
+    MSD_CUDA_CHECK(cudaMemcpyAsync(c->rng_keys, keys.data(), keys.size() * sizeof(uint32_t),
+                                   cudaMemcpyHostToDevice, st));
+    MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+    c->rng_keys_seed = seed;
+  }
+  MSD_TRY(launch_init_z(init_z, c->z, c->z_split, n, c->nd, seed, st, c->cfg.rng_kind, c->rng_keys));
+  MSD_TRY(run_steps(c, noise, seed, 0, mel_out, st));
+  MSD_TRY(end_on(c, caller));
+  return 0;
+}
+
+int msd_sample_rows(msd_ctx* c, const uint64_t* seeds, float* mel_out, void* stream) {
+  MSD_REQUIRE(c && seeds && mel_out, "msd_sample_rows: null argument");
+  MSD_REQUIRE(c->cur_batch > 0, "msd_sample_rows: call msd_encode first");
+  MSD_REQUIRE(c->xrole == 0,
+              "msd_sample_rows: a peer is attached (msd_p2p_attach); the guidance split samples one "
+              "song through msd_sample");
+  const int B = c->cur_batch, steps = c->cfg.num_steps;
+  const long long n_row = static_cast<long long>(c->N) * c->nd;
+  const long long n = B * n_row;
+  const size_t stride = 2 * (static_cast<size_t>(steps) + 1);
+  MSD_REQUIRE(n < (1ll << 32), "msd_sample_rows: %lld elements per call, per-row streams need < 2^32", n);
+  cudaStream_t caller = reinterpret_cast<cudaStream_t>(stream);
+  MSD_TRY(begin_on(c, caller));
+  cudaStream_t st = c->work;
+  // Row b's tables: Philox seed seeds[b], and (jax) PRNGKey(seeds[b]) / fold_in(key, i) exactly as
+  // msd_sample builds them for one seed.  Rows whose seed is unchanged keep their keys.
+  bool dirty = false;
+  std::vector<uint32_t> keys(c->cfg.rng_kind == 1 ? B * stride : 0);
+  for (int b = 0; b < B; ++b) {
+    if (c->row_keys_valid[b] && c->row_seeds_host[b] == seeds[b]) continue;
+    dirty = true;
+    c->row_seeds_host[b] = seeds[b];
+    c->row_keys_valid[b] = 0;  // until the upload below has completed
+    if (c->cfg.rng_kind != 1) continue;
+    uint32_t* k = keys.data() + b * stride;
+    k[0] = static_cast<uint32_t>(seeds[b] >> 32);
+    k[1] = static_cast<uint32_t>(seeds[b]);
+    for (int i = 0; i < steps; ++i)
+      threefry2x32_host(k[0], k[1], 0u, static_cast<uint32_t>(i), &k[2 * (i + 1)]);
+    MSD_CUDA_CHECK(cudaMemcpyAsync(c->row_keys + b * stride, k, stride * sizeof(uint32_t),
+                                   cudaMemcpyHostToDevice, st));
+  }
+  if (dirty) {
+    MSD_CUDA_CHECK(cudaMemcpyAsync(c->row_seeds, c->row_seeds_host.data(),
+                                   static_cast<size_t>(B) * sizeof(unsigned long long),
+                                   cudaMemcpyHostToDevice, st));
+    MSD_CUDA_CHECK(cudaStreamSynchronize(st));  // `keys` is a local
+    for (int b = 0; b < B; ++b) c->row_keys_valid[b] = 1;
+  }
+  MSD_TRY(launch_init_z(nullptr, c->z, c->z_split, n, c->nd, 0, st, c->cfg.rng_kind, c->row_keys,
+                        n_row, static_cast<long long>(stride), c->row_seeds));
+  MSD_TRY(run_steps(c, nullptr, 0, 1, mel_out, st));
   MSD_TRY(end_on(c, caller));
   return 0;
 }

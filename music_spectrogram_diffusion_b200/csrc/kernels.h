@@ -208,6 +208,9 @@ struct RunArgs {
   // ranks; advanced by the sampler kernel) and the counter of blocks that have sent their share
   unsigned int xseq;
   unsigned int xsent;
+  // generated noise drawn per batch row (msd_sample_rows) from SamplerArgs::row_keys / row_seeds
+  // instead of one draw over the whole batch (msd_sample sets 0)
+  int per_row;
 };
 struct SamplerArgs {
   const float* eps;       // [(passes*B)*N, n_dims] rows: cond block then uncond block
@@ -229,6 +232,14 @@ struct SamplerArgs {
   // i + 1 fold_in(key, i)), device memory
   int rng_kind;
   const uint32_t* rng_keys;
+  // per-row streams (run->per_row): element idx of row b = idx / n_row is element idx - b * n_row
+  // of an n_row-element draw from row b's own key table row_keys + b * row_key_stride (same layout
+  // as rng_keys; rng_kind 1) or Philox seed row_seeds[b] (rng_kind 0): the draws that row would
+  // get alone at batch 1.  n_row is a multiple of 8, so a float4 never straddles two rows.
+  long long n_row;
+  const uint32_t* row_keys;
+  long long row_key_stride;
+  const unsigned long long* row_seeds;
   // when non-null: noise / mel_out / seed / step are read from here (device memory) instead of the
   // fields above, and the last block to finish decrements run->step (the step advance)
   RunArgs* run;
@@ -254,10 +265,13 @@ struct SamplerArgs {
 int launch_sampler_step(const SamplerArgs& a, cudaStream_t stream);
 
 // z0 = init (copy or philox normal), plus its [hi | lo | hi] split.
-// rng_kind / rng_keys as in SamplerArgs (keys row 0 is used)
+// rng_kind / rng_keys as in SamplerArgs (keys row 0 is used).  n_row > 0: per-row streams as in
+// SamplerArgs, rng_keys then being the per-row table (row_key_stride words per row) and row_seeds
+// the per-row Philox seeds.
 int launch_init_z(const float* init_z, float* z, bf16* z_split, long long n, int n_dims,
                   unsigned long long seed, cudaStream_t stream, int rng_kind = 0,
-                  const uint32_t* rng_keys = nullptr);
+                  const uint32_t* rng_keys = nullptr, long long n_row = 0,
+                  long long row_key_stride = 0, const unsigned long long* row_seeds = nullptr);
 
 // x[b,t,:] = E[tok[b,t]] + P[t]
 int launch_embed_tokens(const int* tokens, const float* emb, const float* pos, float* x, int B,

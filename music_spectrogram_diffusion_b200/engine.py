@@ -184,6 +184,21 @@ class Engine:
                                       _stream(self.device)), 'msd_sample')
     return out
 
+  def sample_rows(self, seeds, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Like sample(seed=...), but row b of the encoded batch draws its noise from seeds[b] alone:
+    row b comes out as sample(seed=seeds[b]) would draw it at batch 1 (msd_sample_rows)."""
+    seeds = [int(s) for s in seeds]
+    if len(seeds) != self._batch:
+      raise ValueError(f'{len(seeds)} seeds for an encoded batch of {self._batch}')
+    shape = (self._batch, self.cfg.targets_length, self.cfg.n_dims)
+    if out is None:
+      out = torch.empty(shape, dtype=torch.float32, device=self.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape == shape
+    arr = (ctypes.c_uint64 * len(seeds))(*[s & 0xFFFFFFFFFFFFFFFF for s in seeds])
+    _native.check(self.lib.msd_sample_rows(self._h, arr, _ptr(out), _stream(self.device)),
+                  'msd_sample_rows')
+    return out
+
   # -- guidance split over two GPUs (msd_p2p_*, include/msd_b200.h) --------------------------
   def p2p_export(self) -> bytes:
     buf = ctypes.create_string_buffer(64)

@@ -277,15 +277,27 @@ class InferenceModel:
   def predict_on_device(self, tokens: torch.Tensor, ctx_features: torch.Tensor,
                         ctx_mask: torch.Tensor, seed: int = 0,
                         init_z: Optional[torch.Tensor] = None,
-                        noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+                        noise: Optional[torch.Tensor] = None,
+                        seeds: Optional[Sequence[int]] = None) -> torch.Tensor:
     """Device tensors in, device mel out (no host round trip); used by the multi-GPU drivers
-    to hand a segment's prediction to the next segment's context GPU-to-GPU."""
+    to hand a segment's prediction to the next segment's context GPU-to-GPU.
+
+    seeds: one seed per row; row b then draws its noise from seeds[b] alone, i.e. comes out as
+    predict_on_device(row b, seed=seeds[b]) at batch 1 would draw it (Engine.sample_rows), so
+    unrelated segments (e.g. of different songs) can share a batch.  `seed` is then unused, and
+    injected init_z / noise are not accepted."""
     eng = self._get_engine()
     b = tokens.shape[0]
     if b > self.batch_size:
       raise ValueError(f'batch of {b} exceeds batch_size={self.batch_size}')
+    if seeds is not None and (init_z is not None or noise is not None):
+      raise ValueError('per-row seeds draw their own noise: init_z / noise cannot be injected')
+    if seeds is not None and len(seeds) != b:
+      raise ValueError(f'{len(seeds)} seeds for a batch of {b}')
     eng.encode(tokens.to(torch.int32).contiguous(), ctx_features.to(torch.float32).contiguous(),
                ctx_mask.to(torch.int32).contiguous())
+    if seeds is not None:
+      return eng.sample_rows(seeds)
     return eng.sample(init_z, noise, seed=seed).clone()
 
   def predict(self, batch: Mapping[str, np.ndarray], seed: int = 0,
