@@ -284,6 +284,18 @@ int msd_op_jax_normal(uint64_t seed, int32_t step, int64_t n, float* out, void* 
  * out device uint32 [n].  Integer work: the test compares bit-exactly. */
 int msd_op_jax_bits(uint64_t seed, int32_t step, int64_t n, uint32_t* out, void* stream);
 
+/* MelGAN.encode (audio_codecs.py:43-143, 204-247): audio [rows, n_samples] f32 device ->
+ * mel_out [rows, F, 128] f32 device in codec feature units, F = ceil(n_samples / 320).  Frame k
+ * of a row is samples [320 k, 320 k + 640) (zero past the end), times window [640] f32 device
+ * (periodic Hann), zero-padded to 1024; out = log(clip(|rfft| @ mel_weights, 1e-5, 1e8)) with
+ * mel_weights [513, 128] f32 device (linear_to_mel_weight_matrix(128, 513, 16000, 0, 8000)).
+ * Computed in fp32; a frame's output depends on its own 640 samples and the two tables only, so
+ * a song encoded whole and sliced equals the song encoded in pieces.  Refused (-1): a null
+ * pointer, a negative size, or more than 2^31 - 1 output frames; rows = 0 or n_samples = 0
+ * launches nothing.  Asynchronous on `stream`; needs no context. */
+int msd_op_audio_mel(const float* audio, int32_t rows, int64_t n_samples, const float* window,
+                     const float* mel_weights, float* mel_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

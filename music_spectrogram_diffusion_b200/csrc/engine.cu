@@ -1786,6 +1786,19 @@ int msd_op_jax_bits(uint64_t seed, int32_t step, int64_t n, uint32_t* out, void*
   return 0;
 }
 
+int msd_op_audio_mel(const float* audio, int32_t rows, int64_t n_samples, const float* window,
+                     const float* mel_weights, float* mel_out, void* stream) {
+  MSD_REQUIRE(audio && window && mel_weights && mel_out, "msd_op_audio_mel: null argument");
+  MSD_REQUIRE(rows >= 0 && n_samples >= 0, "msd_op_audio_mel: rows=%d, n_samples=%lld must be >= 0",
+              rows, static_cast<long long>(n_samples));
+  const long long frames = audio_mel_frames(n_samples);
+  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
+              "msd_op_audio_mel: %d rows x %lld frames exceed 2^31 - 1 output frames", rows, frames);
+  MSD_TRY(launch_audio_mel(audio, rows, n_samples, window, mel_weights, mel_out,
+                           reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
 int msd_op_dense_epilogue(const float* a, const float* w, const float* w1, int32_t M, int32_t N,
                           int32_t K, int32_t epilogue, int32_t block_n, const float* resid,
                           const float* pos, int32_t pos_rows, const int32_t* pos_shift,

@@ -349,5 +349,10 @@ int launch_bf16_rows_to_f32(const bf16* src, int ld, int lo_off, float* dst, lon
 int launch_jax_normal(uint32_t k0, uint32_t k1, long long n, float* out, cudaStream_t stream);
 // the raw uint32 words the normals above are made from (same in-kernel code path)
 int launch_jax_bits(uint32_t k0, uint32_t k1, long long n, uint32_t* out, cudaStream_t stream);
+// audio [rows, n_samples] f32 -> MelGAN log-mel out [rows, audio_mel_frames(n_samples), 128] f32
+// (audio_mel.cu); window [640], weights [513, 128] f32 device
+long long audio_mel_frames(long long n_samples);
+int launch_audio_mel(const float* audio, int rows, long long n_samples, const float* window,
+                     const float* weights, float* out, cudaStream_t stream);
 
 }  // namespace msd

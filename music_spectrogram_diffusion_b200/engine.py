@@ -425,3 +425,29 @@ def op_jax_normal(seed: int, step: int, n: int, device: torch.device) -> torch.T
   _native.check(_native.load().msd_op_jax_normal(seed, step, n, _ptr(out), _stream(device)),
                 'msd_op_jax_normal')
   return out
+
+
+def op_audio_mel(audio: torch.Tensor, window: torch.Tensor, weights: torch.Tensor) -> torch.Tensor:
+  """MelGAN log-mel features of audio [rows, n] (msd_op_audio_mel): f32 [rows, ceil(n / 320), 128]
+  from the window f32 [640] and mel weights f32 [513, 128] (audio_codecs.mel_tables), all
+  contiguous f32 tensors on one CUDA device.  Enqueued on the device's current stream."""
+  for name, t, shape in (('audio', audio, None), ('window', window, (640,)),
+                         ('weights', weights, (513, 128))):
+    if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+      raise ValueError(f'{name}: expected a contiguous float32 CUDA tensor, got {t.dtype} on '
+                       f'{t.device} (contiguous: {t.is_contiguous()})')
+    if t.device != audio.device:
+      raise ValueError(f'{name} is on {t.device}, audio on {audio.device}')
+    if shape is not None and tuple(t.shape) != shape:
+      raise ValueError(f'{name}: expected shape {shape}, got {tuple(t.shape)}')
+  if audio.dim() != 2:
+    raise ValueError(f'audio: expected [rows, n], got {tuple(audio.shape)}')
+  rows, n = audio.shape
+  out = torch.empty(rows, -(-n // 320), 128, dtype=torch.float32, device=audio.device)
+  if out.numel() == 0:
+    return out
+  with torch.cuda.device(audio.device):
+    _native.check(_native.load().msd_op_audio_mel(_ptr(audio), rows, n, _ptr(window), _ptr(weights),
+                                                   _ptr(out), _stream(audio.device)),
+                  'msd_op_audio_mel')
+  return out

@@ -6,6 +6,11 @@ is conditioned on the previous segment's predicted mel; per-segment wall times a
 with the reference's `model_timing` fields (first segment excluded, evaluation.py:217-220,
 238-247).  The mel -> audio vocoder is outside this path (SURVEY §2).
 
+Audio goes the other way through `MelGAN.encode` (the library's CUDA kernel): `load_audio` reads
+a 16 kHz WAV file, `encode_song_audio` gives a recording's ground-truth mels segment by segment
+(`full_gt_encoded`, evaluation.py:156-276), and `context_audio=` primes a song's first segment
+with the end of a recording instead of a masked-out context.
+
 `synthesize_songs` runs several such chains at once: each round puts the next segment of every
 active song into one batch, one song per row, and every row draws its noise from its own song's
 seed (`InferenceModel.predict_on_device(..., seeds=)`), so a song comes out as it would alone.
@@ -13,7 +18,9 @@ seed (`InferenceModel.predict_on_device(..., seeds=)`), so a song comes out as i
 
 from __future__ import annotations
 
+import io
 import time
+import wave
 from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -39,6 +46,90 @@ def load_notes(midi: Union[str, bytes], sustain: bool = True) -> np.ndarray:
   return song.notes
 
 
+def load_audio(path_or_bytes: Union[str, bytes]) -> np.ndarray:
+  """A 16 kHz PCM WAV file (path or bytes) -> float32 [n] in [-1, 1): 8-bit unsigned, 16-, 24- and
+  32-bit signed samples, scaled by 2^-(bits - 1); channels are averaged to mono as librosa's
+  `load(mono=True)` does.  Any other rate raises ValueError: the reference resamples with librosa,
+  which is not reproduced here, so the audio would not match what the reference encodes."""
+  src = io.BytesIO(path_or_bytes) if isinstance(path_or_bytes, (bytes, bytearray)) else path_or_bytes
+  try:
+    with wave.open(src, 'rb') as w:
+      rate, width, channels = w.getframerate(), w.getsampwidth(), w.getnchannels()
+      raw = w.readframes(w.getnframes())
+  except (wave.Error, EOFError) as e:
+    raise ValueError(f'not a PCM WAV file: {e}') from e
+  if rate != 16000:
+    raise ValueError(f'sample rate {rate} Hz: MelGAN features need 16000 Hz audio, and resampling '
+                     'would not match the reference (librosa); resample before loading')
+  if width == 1:
+    x = (np.frombuffer(raw, np.uint8).astype(np.float32) - 128.0) / 128.0
+  elif width == 2:
+    x = np.frombuffer(raw, '<i2').astype(np.float32) / 32768.0
+  elif width == 3:
+    b = np.frombuffer(raw, np.uint8).reshape(-1, 3).astype(np.int32)
+    v = b[:, 0] | (b[:, 1] << 8) | (b[:, 2] << 16)
+    x = (np.where(v >= 1 << 23, v - (1 << 24), v) / float(1 << 23)).astype(np.float32)
+  elif width == 4:
+    x = (np.frombuffer(raw, '<i4').astype(np.float64) / float(1 << 31)).astype(np.float32)
+  else:
+    raise ValueError(f'{8 * width}-bit samples are not supported (8, 16, 24 or 32-bit PCM)')
+  x = x.reshape(-1, channels)
+  return (x[:, 0] if channels == 1 else x.mean(axis=1, dtype=np.float32)).astype(np.float32)
+
+
+def encode_song_audio(model, samples: np.ndarray) -> Dict[str, Any]:
+  """A song's recording -> its ground-truth mels, as the reference's full-song evaluation cuts them
+  (`split_full_song` + `encode_audio`, preprocessors.py:60-81, 631-696, 863-921).
+
+  The samples are padded by 320 - n % 320 (a whole hop when n is a multiple), giving num_frames
+  hop-frames (`midi_tokens.num_song_frames`); segment s is frames [s * targets, (s + 1) * targets)
+  encoded with the 16 frames after it, and the last one is padded with 0.0 to a full segment.  A
+  frame depends on its own 640 samples only, so the song is encoded once and cut.
+  Returns {'full_gt_encoded': f32 [segments * targets, n_dims], 'num_frames': int}."""
+  ac = model.audio_codec
+  per_segment = model.sequence_length['targets']
+  x = np.asarray(samples, np.float32)
+  if x.ndim != 1:
+    raise ValueError(f'samples must be 1-D, got shape {x.shape}')
+  x = np.pad(x, [0, ac.hop_size - len(x) % ac.hop_size])
+  total = len(x) // ac.hop_size
+  full = np.zeros((-(-total // per_segment) * per_segment, ac.n_dims), np.float32)
+  full[:total] = ac.encode(x)
+  return {'full_gt_encoded': full, 'num_frames': total}
+
+
+def primer_frames(n_samples: int, context_frames: int, hop: int = 320,
+                  window: int = 640) -> Tuple[int, int]:
+  """(first, count): the recording's frames [first, first + count) that prime a song -- the last
+  min(context_frames, n_samples // hop - 1) frames whose whole window lies inside the recording,
+  as every context frame of training had real audio under it."""
+  if n_samples < window:
+    raise ValueError(f'a context recording needs at least {window} samples, got {n_samples}')
+  usable = n_samples // hop - 1
+  count = min(context_frames, usable)
+  return usable - count, count
+
+
+def audio_context(model, audio, device: Optional[torch.device] = None
+                  ) -> Tuple[torch.Tensor, torch.Tensor]:
+  """A recording (f32 [n] at 16 kHz, numpy or tensor) -> (ctx f32 [1, C, n_dims], mask int32
+  [1, C]) on `device` (default: the model's): its last frames (`primer_frames`) front-filled,
+  mask 1 over them and 0 after (the feature converter's sequence_mask layout)."""
+  ac = model.audio_codec
+  c = model.sequence_length.get('targets_context') or 0
+  device = model.engine.device if device is None else device
+  a = torch.as_tensor(audio).to(device, torch.float32).contiguous()
+  if a.dim() != 1:
+    raise ValueError(f'context audio must be 1-D, got shape {tuple(a.shape)}')
+  first, count = primer_frames(a.shape[0], c, ac.hop_size)
+  span = a[first * ac.hop_size:(first + count + 1) * ac.hop_size]
+  ctx = torch.zeros(1, c, ac.n_dims, dtype=torch.float32, device=device)
+  ctx[0, :count] = ac.encode(span)[:count]
+  mask = torch.zeros(1, c, dtype=torch.int32, device=device)
+  mask[0, :count] = 1
+  return ctx, mask
+
+
 def _tokenize(model, notes: np.ndarray, max_segments: Optional[int]):
   """(tokenize_song result, number of segments to synthesise)."""
   ac = model.audio_codec
@@ -52,8 +143,10 @@ def _tokenize(model, notes: np.ndarray, max_segments: Optional[int]):
 
 
 def synthesize_song(model, notes: np.ndarray, seed: int = 0, always_mask_context: bool = False,
-                    max_segments: Optional[int] = None) -> Dict[str, Any]:
+                    max_segments: Optional[int] = None, context_audio=None) -> Dict[str, Any]:
   """model: an `InferenceModel` (anything with .predict, .sequence_length, .audio_codec, .codec).
+  context_audio: a 16 kHz recording (f32 [n], at least 640 samples) whose end conditions the first
+  segment (`audio_context`) instead of a masked-out context; not with always_mask_context.
 
   Returns {'full_pred_encoded': f32 [segments * targets_length, n_dims] in feature units,
   'num_frames': frames that belong to the song, 'tokens': the per-segment model inputs,
@@ -63,15 +156,21 @@ def synthesize_song(model, notes: np.ndarray, seed: int = 0, always_mask_context
   toks, nseg = _tokenize(model, notes, max_segments)
   ctx_len = lengths.get('targets_context') or 0
   pred = np.zeros((1, ctx_len, ac.n_dims), np.float32)
+  primer_mask = None
+  if context_audio is not None:
+    if always_mask_context:
+      raise ValueError('context_audio with always_mask_context: the context would be masked out')
+    pred, primer_mask = (t.cpu().numpy() for t in audio_context(model, context_audio))
   full = np.zeros((1, 0, ac.n_dims), np.float32)
   seconds = []
   for i in range(nseg):
     batch = {
         'encoder_input_tokens': toks.tokens[i:i + 1],
         'encoder_continuous_inputs': pred[:1],
-        # first segment: nothing to condition on; later ones: a full chunk of predicted context
-        'encoder_continuous_mask': (np.zeros if (i == 0 or always_mask_context) else np.ones)(
-            (1, ctx_len), np.int32),
+        # first segment: nothing to condition on (or the recording); later ones: a full chunk of
+        # predicted context
+        'encoder_continuous_mask': primer_mask if (i == 0 and primer_mask is not None) else (
+            np.zeros if (i == 0 or always_mask_context) else np.ones)((1, ctx_len), np.int32),
         'decoder_target_tokens': np.zeros((1, lengths['targets'], ac.n_dims), np.float32),
     }
     tick = time.time()
@@ -94,7 +193,9 @@ def synthesize_song(model, notes: np.ndarray, seed: int = 0, always_mask_context
 
 def chain_songs(predict_rows: PredictRows, token_segments: Sequence[torch.Tensor], slots: int,
                 context_frames: int, n_dims: int, device: torch.device, seeds: Sequence[int],
-                always_mask_context: bool = False) -> Tuple[List[torch.Tensor], List[Dict[str, Any]]]:
+                always_mask_context: bool = False,
+                initial_context: Optional[Sequence[Optional[Tuple[torch.Tensor, torch.Tensor]]]] = None
+                ) -> Tuple[List[torch.Tensor], List[Dict[str, Any]]]:
   """Chained synthesis of several songs, batched across rows (the scheduling core of
   `synthesize_songs`).
 
@@ -103,7 +204,9 @@ def chain_songs(predict_rows: PredictRows, token_segments: Sequence[torch.Tensor
   soon as a slot is free, in order, and contributes its next segment to every round until it is
   done.  A row's context is its song's previous prediction, kept on `device`; a song's first
   segment (every segment with always_mask_context) gets an all-zero mask, later ones all-one
-  masks (beam/evaluation.py:187-203).
+  masks (beam/evaluation.py:187-203).  initial_context[s], when given and not None, is song s's
+  (ctx f32 [1, context_frames, n_dims], mask int32 [1, context_frames]) on `device`, used for its
+  first segment instead of the masked-out context (`audio_context`).
 
   Returns (mel [1, n_segments_s * frames, n_dims] per song, rounds), rounds[k] = {'rows': [(song,
   segment), ...], 'seconds': host wall time of the round, synchronised with the device when the
@@ -113,7 +216,18 @@ def chain_songs(predict_rows: PredictRows, token_segments: Sequence[torch.Tensor
   if len(seeds) != len(token_segments):
     raise ValueError(f'{len(seeds)} seeds for {len(token_segments)} songs')
   n_songs = len(token_segments)
+  if initial_context is not None:
+    if len(initial_context) != n_songs:
+      raise ValueError(f'{len(initial_context)} initial contexts for {n_songs} songs')
+    if always_mask_context and any(c is not None for c in initial_context):
+      raise ValueError('an initial context with always_mask_context: it would be masked out')
+    for c in initial_context:
+      if c is not None and (tuple(c[0].shape) != (1, context_frames, n_dims)
+                            or tuple(c[1].shape) != (1, context_frames)):
+        raise ValueError(f'an initial context must be ([1, {context_frames}, {n_dims}], '
+                         f'[1, {context_frames}]), got {tuple(c[0].shape)}, {tuple(c[1].shape)}')
   done = [0] * n_songs
+  primed = lambda s: initial_context is not None and initial_context[s] is not None and done[s] == 0
   prev: List[Optional[torch.Tensor]] = [None] * n_songs
   outs: List[List[torch.Tensor]] = [[] for _ in range(n_songs)]
   rounds: List[Dict[str, Any]] = []
@@ -128,10 +242,14 @@ def chain_songs(predict_rows: PredictRows, token_segments: Sequence[torch.Tensor
       break
     toks = torch.stack([token_segments[s][done[s]] for s in active]).to(device, torch.int32)
     zero = torch.zeros(1, context_frames, n_dims, dtype=torch.float32, device=device)
-    ctx = torch.cat([zero if prev[s] is None else prev[s] for s in active])
+    ctx = torch.cat([initial_context[s][0] if primed(s) else zero if prev[s] is None else prev[s]
+                     for s in active])
     first = [done[s] == 0 or always_mask_context for s in active]
     mask = torch.tensor([[0 if f else 1] for f in first], dtype=torch.int32,
                         device=device).expand(len(active), context_frames).contiguous()
+    if any(primed(s) for s in active):
+      mask = torch.cat([initial_context[s][1].to(torch.int32) if primed(s) else mask[r:r + 1]
+                        for r, s in enumerate(active)])
     if toks.is_cuda:
       torch.cuda.synchronize(device)
     tick = time.time()
@@ -149,12 +267,15 @@ def chain_songs(predict_rows: PredictRows, token_segments: Sequence[torch.Tensor
 
 
 def synthesize_songs(model, songs: Sequence[np.ndarray], seeds: Optional[Sequence[int]] = None,
-                     always_mask_context: bool = False, max_segments: Optional[int] = None
+                     always_mask_context: bool = False, max_segments: Optional[int] = None,
+                     context_audios: Optional[Sequence[Any]] = None
                      ) -> Tuple[List[Dict[str, Any]], Dict[str, float]]:
   """`synthesize_song` for many songs at once: up to model.batch_size songs run side by side, one
   per batch row (`chain_songs`), each drawing its noise from its own seed, so every song comes out
   as `synthesize_song(model, notes, seed)` computes it up to the kernels' batch-size dependent
   rounding.  seeds: one per song, default 0 for every song (the reference's `predict(batch)`).
+  context_audios: one recording or None per song, as synthesize_song's context_audio; the
+  recordings are encoded on the device and stay there.
 
   Returns (one dict per song with synthesize_song's keys, aggregate): model_timing of a song is
   the mean wall time of the rounds that carried its segments after its first; aggregate =
@@ -164,16 +285,23 @@ def synthesize_songs(model, songs: Sequence[np.ndarray], seeds: Optional[Sequenc
     seeds = [0] * len(songs)
   if len(seeds) != len(songs):
     raise ValueError(f'{len(seeds)} seeds for {len(songs)} songs')
+  if context_audios is not None and len(context_audios) != len(songs):
+    raise ValueError(f'{len(context_audios)} context recordings for {len(songs)} songs')
+  if always_mask_context and context_audios is not None and any(
+      a is not None for a in context_audios):
+    raise ValueError('context_audios with always_mask_context: the context would be masked out')
   ac = model.audio_codec
   lengths = model.sequence_length
   device = model.engine.device
+  primers = None if context_audios is None else [
+      None if a is None else audio_context(model, a, device) for a in context_audios]
   tokenized = [_tokenize(model, notes, max_segments) for notes in songs]
   segs = [torch.from_numpy(np.ascontiguousarray(t.tokens[:n], dtype=np.int32)).to(device)
           for t, n in tokenized]
   mels, rounds = chain_songs(
       lambda toks, ctx, mask, row_seeds: model.predict_on_device(toks, ctx, mask, seeds=row_seeds),
       segs, model.batch_size, lengths.get('targets_context') or 0, ac.n_dims, device,
-      [int(s) for s in seeds], always_mask_context)
+      [int(s) for s in seeds], always_mask_context, primers)
   seconds_per_chunk = lengths['targets'] * (ac.hop_size / ac.sample_rate)
   later: List[List[float]] = [[] for _ in songs]
   for rd in rounds:
