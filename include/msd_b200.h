@@ -296,6 +296,27 @@ int msd_op_jax_bits(uint64_t seed, int32_t step, int64_t n, uint32_t* out, void*
 int msd_op_audio_mel(const float* audio, int32_t rows, int64_t n_samples, const float* window,
                      const float* mel_weights, float* mel_out, void* stream);
 
+/* Resampling of recordings to the codec's rate as the reference does it (preprocessors.py:150-155,
+ * 332-333, 518-521: librosa.resample(y, sr, 16000) and librosa.load(sr=16000), i.e. librosa 0.9
+ * res_type='kaiser_best' = resampy 0.2.2 `resample_f`): x [rows, n_in] f32 device -> y [rows,
+ * n_out] f32 device, n_out = int(n_in * ((double)target_sr / orig_sr)) (resampy's length; the
+ * caller zero-pads to librosa's ceil).  half_window [window_len] f64 device is the unscaled filter
+ * half (kaiser_best: 32769 entries), scaled by the ratio when downsampling as resampy does.
+ * precision is log2 of the window's entries per zero crossing: 9 for kaiser_best, whose
+ * get_filter returns num_table = 2^9 = 512 (resampy passes that to resample_f).  time_segments [n_segments, 3] f64 device
+ * (t_s, r_s, d), t_s ascending from 0, describe resampy's running float64 time register: for
+ * t_s <= t < t_{s+1}, r_t = r_s + (t - t_s) d exactly (audio_codecs.time_register_segments).
+ * Every tap is a float64 multiply and add rounded to float32, in resampy's order: the result is
+ * bit for bit the sequential loop's.  Refused (-1): a null pointer, a negative size, a rate <= 0,
+ * an n_out other than the length above, more than 65535 rows or 2^31 - 1 samples in or out, a
+ * precision outside 0..24, window_len < 2, n_segments < 1, or a ratio below one window entry per
+ * input sample.  rows = 0 or n_out = 0 launches nothing.  Asynchronous on `stream`; needs no
+ * context. */
+int msd_op_audio_resample(const float* x, int32_t rows, int64_t n_in, int32_t orig_sr,
+                          int32_t target_sr, const double* half_window, int32_t window_len,
+                          int32_t precision, const double* time_segments, int32_t n_segments,
+                          float* y, int64_t n_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

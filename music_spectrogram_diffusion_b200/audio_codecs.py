@@ -5,16 +5,30 @@ MelGAN constants (204-218).  `MelGAN.encode` is the reference's Audio2Mel (43-14
 settings (226-247), computed by the library's CUDA kernel (`engine.op_audio_mel`) from the float32
 tables built here (`hann_window`, `linear_to_mel_weight_matrix`, in TF's order of operations).
 The vocoder (`decode`, a TF-Hub SavedModel, 249-264) is out of scope: it raises.
+
+Recordings at other rates are brought to 16 kHz by `resample`, librosa 0.9's
+`resample(res_type='kaiser_best')` as the reference calls it (preprocessors.py:150-155, 332-333,
+518-521), computed by the library's CUDA kernel (`engine.op_audio_resample`) bit for bit as
+resampy 0.2.2's loop, from the filter built here (`kaiser_best_window`) and the time register
+described by `time_register_segments`.
 """
 
 from __future__ import annotations
 
+import math
 from typing import Dict, Tuple
 
 import numpy as np
 
 MEL_WIN_LENGTH = 640    # MelGAN._frame_length
 MEL_FFT_SIZE = 1024     # MelGAN._fft_size
+
+# resampy's 'kaiser_best' filter: sinc_window(num_zeros=64, precision=9,
+# window=kaiser(beta=14.769656459379492), rolloff=0.9475937167399596)
+KAISER_BEST_NUM_ZEROS = 64
+KAISER_BEST_PRECISION = 9
+KAISER_BEST_BETA = 14.769656459379492
+KAISER_BEST_ROLLOFF = 0.9475937167399596
 
 
 def hann_window(length: int = MEL_WIN_LENGTH) -> np.ndarray:
@@ -68,6 +82,124 @@ def mel_tables(device):
             MelGAN.n_dims, MEL_FFT_SIZE // 2 + 1, MelGAN.sample_rate, 0.0,
             float(MelGAN.sample_rate // 2))).to(device))
   return _DEVICE_TABLES[device]
+
+
+_KAISER_BEST = []
+_DEVICE_WINDOWS: Dict[object, object] = {}
+
+
+def kaiser_best_window() -> np.ndarray:
+  """resampy's 'kaiser_best' half window, f64 [64 * 2^9 + 1] (read-only):
+  rolloff * sinc(rolloff * linspace(0, 64, 32769)) * kaiser(65537, beta)[32768:], with numpy's
+  sinc and kaiser.  resampy ships the same table precomputed (data/kaiser_best.npz); the two may
+  differ in their last bits (DESIGN section 4)."""
+  if not _KAISER_BEST:
+    n = (1 << KAISER_BEST_PRECISION) * KAISER_BEST_NUM_ZEROS
+    sinc = KAISER_BEST_ROLLOFF * np.sinc(
+        KAISER_BEST_ROLLOFF * np.linspace(0, KAISER_BEST_NUM_ZEROS, num=n + 1, endpoint=True))
+    win = np.kaiser(2 * n + 1, KAISER_BEST_BETA)[n:] * sinc
+    win.setflags(write=False)
+    _KAISER_BEST.append(win)
+  return _KAISER_BEST[0]
+
+
+def resample_window(device):
+  """`kaiser_best_window()` as a float64 tensor on `device`, built once per device."""
+  if device not in _DEVICE_WINDOWS:
+    import torch
+    _DEVICE_WINDOWS[device] = torch.from_numpy(kaiser_best_window().copy()).to(device)
+  return _DEVICE_WINDOWS[device]
+
+
+def resampy_length(n: int, orig_sr: int, target_sr: int) -> int:
+  """resampy's output length, int(n * target / orig) in float64."""
+  return int(n * (float(target_sr) / orig_sr))
+
+
+def librosa_length(n: int, orig_sr: int, target_sr: int) -> int:
+  """librosa.resample's output length, ceil(n * target / orig) in float64 (fix=True pads the
+  resampy output with zeros to it)."""
+  return int(np.ceil(n * (float(target_sr) / orig_sr)))
+
+
+def time_register_segments(orig_sr: int, target_sr: int, n_out: int) -> np.ndarray:
+  """resampy's time register r_0 = 0, r_{t+1} = fl(r_t + 1 / ratio) for t < n_out, as f64 [S, 3]
+  rows (t_s, r_s, d): for t_s <= t < t_{s+1} (t_{S} = n_out), r_t = r_s + (t - t_s) d exactly.
+
+  While r stays inside one binade [2^e, 2^(e+1)) every r is a multiple of that binade's ulp u,
+  so fl(r + inc) = r + d with d = inc rounded to a multiple of u -- the same d for every step,
+  unless inc is an exact tie on that grid (round-half-even then depends on r).  A segment is
+  such a run of steps, ended short of the binade's top; steps near the top, ties and r = 0 get
+  segments of one output.  That gives about three segments per binade of the output's span."""
+  inc = 1.0 / (float(target_sr) / orig_sr)
+  segs = []
+  t, r = 0, 0.0
+  while t < n_out:
+    d = (r + inc) - r
+    length = 1
+    if r > 0.0:
+      e = math.frexp(r)[1]                  # r in [2^(e-1), 2^e)
+      top, u = math.ldexp(1.0, e), math.ldexp(1.0, e - 53)
+      if math.fmod(inc, u) != u / 2:
+        # steps j < length - 1 keep r + j d + inc below top: fl adds exactly d
+        length = max(1, int((top - r) / d) - 1)
+    length = min(length, n_out - t)
+    segs.append((t, r, d))
+    t += length
+    r = (r + (length - 1) * d) + inc
+  return np.array(segs, np.float64).reshape(-1, 3)
+
+
+def resample(audio, orig_sr: int, target_sr: int = 16000):
+  """librosa 0.9 `resample(audio, orig_sr, target_sr)` with its default res_type='kaiser_best':
+  float32 audio [n] or [rows, n] -> [(rows,) ceil(n * target_sr / orig_sr)] float32, each row
+  resampled by resampy's band-limited sinc interpolation and zero-padded at the end to librosa's
+  length.  Equal rates return `audio` unchanged, as librosa does.  Computed on the GPU with
+  float64 taps into a float32 result, bit for bit resampy's loop on float32 samples (what
+  librosa.load reads; `engine.op_audio_resample`).  Other dtypes are refused rather than rounded:
+  librosa keeps float64 samples in float64, which this is not.  A numpy array is resampled on the
+  current CUDA device and comes back as numpy; a CUDA tensor stays on its device.  Raises
+  ValueError for rates <= 0, a dtype other than float32 and, as resampy does, when
+  int(n * ratio) < 1."""
+  import torch
+  from music_spectrogram_diffusion_b200 import engine
+  if int(orig_sr) != orig_sr or int(target_sr) != target_sr or orig_sr <= 0 or target_sr <= 0:
+    raise ValueError(f'resample: rates must be positive integers, got {orig_sr} -> {target_sr}')
+  orig_sr, target_sr = int(orig_sr), int(target_sr)
+  as_numpy = not torch.is_tensor(audio)
+  if as_numpy:
+    audio = np.asarray(audio)
+  elif not audio.is_cuda:
+    raise ValueError('resample: a tensor must be on a CUDA device (or pass numpy)')
+  if audio.ndim not in (1, 2):
+    raise ValueError(f'resample: audio must be [n] or [rows, n], got {tuple(audio.shape)}')
+  if audio.dtype not in (np.float32, torch.float32):
+    raise ValueError(f'resample: audio must be float32 (librosa.load reads float32; cast first), '
+                     f'got {audio.dtype}')
+  if orig_sr == target_sr:
+    return audio
+  n = audio.shape[-1]
+  n_out = resampy_length(n, orig_sr, target_sr)
+  if n_out < 1:
+    raise ValueError(f'resample: {n} samples at {orig_sr} Hz give no output at {target_sr} Hz')
+  segs = time_register_segments(orig_sr, target_sr, n_out)
+  t_s, r_s, d = segs[-1]
+  if int(r_s + (n_out - 1 - t_s) * d) >= n:
+    raise ValueError(f'resample: {n} samples are too long for the float64 time register '
+                     f'at {orig_sr} -> {target_sr} Hz: it runs past the input')
+  if as_numpy:
+    dev = torch.device('cuda', torch.cuda.current_device())
+    x = torch.from_numpy(np.ascontiguousarray(audio)).to(dev)
+  else:
+    dev = audio.device
+    x = audio
+  rows = (x if x.dim() == 2 else x[None]).contiguous()
+  y = engine.op_audio_resample(rows, orig_sr, target_sr, resample_window(dev),
+                               KAISER_BEST_PRECISION, torch.from_numpy(segs).to(dev))
+  y = torch.nn.functional.pad(y, (0, librosa_length(n, orig_sr, target_sr) - n_out))
+  if audio.ndim == 1:
+    y = y[0]
+  return y.cpu().numpy() if as_numpy else y
 
 
 class AudioCodec:

@@ -1799,6 +1799,36 @@ int msd_op_audio_mel(const float* audio, int32_t rows, int64_t n_samples, const 
   return 0;
 }
 
+int msd_op_audio_resample(const float* x, int32_t rows, int64_t n_in, int32_t orig_sr,
+                          int32_t target_sr, const double* half_window, int32_t window_len,
+                          int32_t precision, const double* time_segments, int32_t n_segments,
+                          float* y, int64_t n_out, void* stream) {
+  MSD_REQUIRE(x && half_window && time_segments && y, "msd_op_audio_resample: null argument");
+  MSD_REQUIRE(rows >= 0 && n_in >= 0 && n_out >= 0,
+              "msd_op_audio_resample: rows=%d, n_in=%lld, n_out=%lld must be >= 0", rows,
+              static_cast<long long>(n_in), static_cast<long long>(n_out));
+  MSD_REQUIRE(orig_sr > 0 && target_sr > 0, "msd_op_audio_resample: rates %d -> %d must be > 0",
+              orig_sr, target_sr);
+  const double ratio = static_cast<double>(target_sr) / orig_sr;
+  const long long want = static_cast<long long>(static_cast<double>(n_in) * ratio);
+  MSD_REQUIRE(n_out == want, "msd_op_audio_resample: n_out=%lld, int(n_in * ratio) is %lld",
+              static_cast<long long>(n_out), want);
+  MSD_REQUIRE(n_in <= INT32_MAX && n_out <= INT32_MAX && rows <= 65535,
+              "msd_op_audio_resample: %d rows x %lld -> %lld samples: at most 65535 rows of "
+              "2^31 - 1 samples", rows, static_cast<long long>(n_in), static_cast<long long>(n_out));
+  MSD_REQUIRE(precision >= 0 && precision <= 24 && window_len >= 2 && n_segments >= 1,
+              "msd_op_audio_resample: precision=%d (0..24), window_len=%d (>= 2), "
+              "n_segments=%d (>= 1)", precision, window_len, n_segments);
+  const int num_table = 1 << precision;
+  MSD_REQUIRE(static_cast<int>((ratio < 1.0 ? ratio : 1.0) * num_table) >= 1,
+              "msd_op_audio_resample: %d -> %d Hz is below one window entry per input sample",
+              orig_sr, target_sr);
+  MSD_TRY(launch_audio_resample(x, rows, static_cast<int>(n_in), ratio, half_window, window_len,
+                                num_table, time_segments, n_segments, y, static_cast<int>(n_out),
+                                reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
 int msd_op_dense_epilogue(const float* a, const float* w, const float* w1, int32_t M, int32_t N,
                           int32_t K, int32_t epilogue, int32_t block_n, const float* resid,
                           const float* pos, int32_t pos_rows, const int32_t* pos_shift,

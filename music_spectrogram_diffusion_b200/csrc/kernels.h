@@ -354,5 +354,11 @@ int launch_jax_bits(uint32_t k0, uint32_t k1, long long n, uint32_t* out, cudaSt
 long long audio_mel_frames(long long n_samples);
 int launch_audio_mel(const float* audio, int rows, long long n_samples, const float* window,
                      const float* weights, float* out, cudaStream_t stream);
+// x [rows, n_in] f32 -> y [rows, n_out] f32 resampled by ratio = target / orig as resampy's
+// resample_f (audio_resample.cu); window [window_len] f64 unscaled half window with num_table
+// entries per zero crossing, segments [n_segments, 3] f64 (t_s, r_s, d) of the time register
+int launch_audio_resample(const float* x, int rows, int n_in, double ratio, const double* window,
+                          int window_len, int num_table, const double* segments, int n_segments,
+                          float* y, int n_out, cudaStream_t stream);
 
 }  // namespace msd

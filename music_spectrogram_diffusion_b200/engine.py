@@ -451,3 +451,37 @@ def op_audio_mel(audio: torch.Tensor, window: torch.Tensor, weights: torch.Tenso
                                                    _ptr(out), _stream(audio.device)),
                   'msd_op_audio_mel')
   return out
+
+
+def op_audio_resample(audio: torch.Tensor, orig_sr: int, target_sr: int, window: torch.Tensor,
+                      precision: int, segments: torch.Tensor) -> torch.Tensor:
+  """audio [rows, n] resampled from orig_sr to target_sr as resampy's kaiser_best loop does it
+  (msd_op_audio_resample): f32 [rows, int(n * target_sr / orig_sr)] (resampy's length, not yet
+  padded to librosa's).  audio is a contiguous f32 CUDA tensor; window (the unscaled half window,
+  audio_codecs.resample_window) f64 [window_len] with 2^precision entries per zero crossing, and
+  segments (audio_codecs.time_register_segments) f64 [S, 3], on the same device.  Enqueued on the
+  device's current stream."""
+  for name, t, dtype, dim in (('audio', audio, torch.float32, 2), ('window', window, torch.float64, 1),
+                              ('segments', segments, torch.float64, 2)):
+    if t.dtype != dtype or not t.is_cuda or not t.is_contiguous():
+      raise ValueError(f'{name}: expected a contiguous {dtype} CUDA tensor, got {t.dtype} on '
+                       f'{t.device} (contiguous: {t.is_contiguous()})')
+    if t.device != audio.device:
+      raise ValueError(f'{name} is on {t.device}, audio on {audio.device}')
+    if t.dim() != dim:
+      raise ValueError(f'{name}: expected {dim} dimensions, got {tuple(t.shape)}')
+  if segments.shape[1] != 3 or segments.shape[0] < 1:
+    raise ValueError(f'segments: expected [S >= 1, 3], got {tuple(segments.shape)}')
+  if int(orig_sr) != orig_sr or int(target_sr) != target_sr or orig_sr <= 0 or target_sr <= 0:
+    raise ValueError(f'rates must be positive integers, got {orig_sr} -> {target_sr}')
+  rows, n = audio.shape
+  out = torch.empty(rows, int(n * (float(target_sr) / orig_sr)), dtype=torch.float32,
+                    device=audio.device)
+  if out.numel() == 0:
+    return out
+  with torch.cuda.device(audio.device):
+    _native.check(_native.load().msd_op_audio_resample(
+        _ptr(audio), rows, n, int(orig_sr), int(target_sr), _ptr(window), window.shape[0],
+        precision, _ptr(segments), segments.shape[0], _ptr(out), out.shape[1],
+        _stream(audio.device)), 'msd_op_audio_resample')
+  return out

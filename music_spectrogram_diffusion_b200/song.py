@@ -7,7 +7,8 @@ with the reference's `model_timing` fields (first segment excluded, evaluation.p
 238-247).  The mel -> audio vocoder is outside this path (SURVEY §2).
 
 Audio goes the other way through `MelGAN.encode` (the library's CUDA kernel): `load_audio` reads
-a 16 kHz WAV file, `encode_song_audio` gives a recording's ground-truth mels segment by segment
+a 16 kHz WAV file (or, with resample=True, a WAV file at any rate, resampled to 16 kHz on the GPU
+as the reference's librosa does), `encode_song_audio` gives a recording's ground-truth mels segment by segment
 (`full_gt_encoded`, evaluation.py:156-276), and `context_audio=` primes a song's first segment
 with the end of a recording instead of a masked-out context.
 
@@ -26,7 +27,7 @@ from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 import torch
 
-from music_spectrogram_diffusion_b200 import midi_file, midi_tokens
+from music_spectrogram_diffusion_b200 import audio_codecs, midi_file, midi_tokens
 
 # predict_rows(tokens [R, inputs], ctx [R, context, n_dims], mask [R, context], seeds: R ints)
 #   -> mel [R, targets, n_dims]; row r must depend on row r of the inputs and seeds[r] only
@@ -46,11 +47,16 @@ def load_notes(midi: Union[str, bytes], sustain: bool = True) -> np.ndarray:
   return song.notes
 
 
-def load_audio(path_or_bytes: Union[str, bytes]) -> np.ndarray:
-  """A 16 kHz PCM WAV file (path or bytes) -> float32 [n] in [-1, 1): 8-bit unsigned, 16-, 24- and
-  32-bit signed samples, scaled by 2^-(bits - 1); channels are averaged to mono as librosa's
-  `load(mono=True)` does.  Any other rate raises ValueError: the reference resamples with librosa,
-  which is not reproduced here, so the audio would not match what the reference encodes."""
+def load_audio(path_or_bytes: Union[str, bytes], resample: bool = False) -> np.ndarray:
+  """A PCM WAV file (path or bytes) -> float32 [n] at 16 kHz in [-1, 1): 8-bit unsigned, 16-, 24-
+  and 32-bit signed samples, scaled by 2^-(bits - 1); channels are averaged to mono as librosa's
+  `load(mono=True)` does.
+
+  By default the file must be at 16 kHz; any other rate raises ValueError.  With resample=True a
+  file at any rate is read and mixed down the same way, then resampled to 16 kHz on the GPU as
+  `librosa.load(sr=16000)` does (`audio_codecs.resample`: librosa 0.9's kaiser_best, bit for bit
+  resampy's loop; preprocessors.py:150-155, 332-333, 518-521).  A 16 kHz file comes back
+  unchanged."""
   src = io.BytesIO(path_or_bytes) if isinstance(path_or_bytes, (bytes, bytearray)) else path_or_bytes
   try:
     with wave.open(src, 'rb') as w:
@@ -58,9 +64,9 @@ def load_audio(path_or_bytes: Union[str, bytes]) -> np.ndarray:
       raw = w.readframes(w.getnframes())
   except (wave.Error, EOFError) as e:
     raise ValueError(f'not a PCM WAV file: {e}') from e
-  if rate != 16000:
-    raise ValueError(f'sample rate {rate} Hz: MelGAN features need 16000 Hz audio, and resampling '
-                     'would not match the reference (librosa); resample before loading')
+  if rate != 16000 and not resample:
+    raise ValueError(f'sample rate {rate} Hz: MelGAN features need 16000 Hz audio; pass '
+                     'resample=True to resample it as the reference does (librosa)')
   if width == 1:
     x = (np.frombuffer(raw, np.uint8).astype(np.float32) - 128.0) / 128.0
   elif width == 2:
@@ -74,7 +80,10 @@ def load_audio(path_or_bytes: Union[str, bytes]) -> np.ndarray:
   else:
     raise ValueError(f'{8 * width}-bit samples are not supported (8, 16, 24 or 32-bit PCM)')
   x = x.reshape(-1, channels)
-  return (x[:, 0] if channels == 1 else x.mean(axis=1, dtype=np.float32)).astype(np.float32)
+  x = (x[:, 0] if channels == 1 else x.mean(axis=1, dtype=np.float32)).astype(np.float32)
+  if rate != 16000:
+    x = audio_codecs.resample(x, rate, 16000)
+  return x
 
 
 def encode_song_audio(model, samples: np.ndarray) -> Dict[str, Any]:
