@@ -270,6 +270,54 @@ int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq
                           int32_t o_ld, float* part_o, float* part_ml, int32_t splits, int32_t tail,
                           void* stream);
 
+/* The GEMM on caller-owned device buffers, launched with every argument the engine's decoder sets
+ * (views into fused buffers, step-indexed tables, deferred normalisation):
+ *   a, b        bf16 operands as element offset + leading dimension: out = A[M, K] B[N, K]^T.
+ *   epilogue    0 bf16, 1 f32, 2 f32 + resid, 3 gated GELU (bf16 [M, N / 2]), 4 f32 + position rows,
+ *               5 gated GELU split [hi | lo | hi] (bf16 [M, 3 N / 2]), 6 deferred-normalisation
+ *               producer (out == resid, f32 in place; see msd_op_dense_deferred_norm).
+ *   block_n     0 = automatic, else 64 / 96 / 128 / 192 / 256; variant as in msd_op_dense_variant.
+ *   out         f32 (epilogues 1, 2, 4, 6) or bf16 (0, 3, 5) at element offset out_off, row stride ldo;
+ *               resid f32 at resid_off with the same ldo, or NULL.
+ *   pos / pos_rows / pos_shift / dup_rows   epilogue 4, as in msd_op_dense_epilogue.
+ *   step        device int32 diffusion step index the *_step_stride arguments multiply, or NULL.
+ *   prep_*      epilogue 6: column gains g_lo (rows < prep_split_row) / g_hi at base + step * stride,
+ *               bf16 operand written to prep_a [M, prep_lda], row sums of squares of each column tile
+ *               t written to prep_ss[t * prep_ss_stride + row].
+ *   rs_*        epilogues 0 / 3 (rs_ss_lo != NULL): row r's accumulator is scaled by
+ *               rsqrt(inv_d * sum_{t < parts} ss[t * rs_ss_stride + r] + 1e-6), ss / parts = the _lo
+ *               pair for r < rs_split_row, else the _hi pair; then rs_col_bias + step * stride is added.
+ * *block_n_out (host, may be NULL) receives the tile width that ran: epilogue 6 writes N / width
+ * partial sums per row.  The launch waits for all earlier work on the stream; synchronises it. */
+int msd_op_gemm_view(const void* a, int64_t a_off, int32_t lda, const void* b, int64_t b_off, int32_t ldb,
+                     int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n, int32_t variant,
+                     void* out, int64_t out_off, int32_t ldo, const float* resid, int64_t resid_off,
+                     const float* pos, int32_t pos_rows, const int32_t* pos_shift, int32_t dup_rows,
+                     const int32_t* step, const float* prep_g_lo, int64_t prep_g_lo_step_stride,
+                     const float* prep_g_hi, int64_t prep_g_hi_step_stride, int32_t prep_split_row,
+                     void* prep_a, int32_t prep_lda, float* prep_ss, int32_t prep_ss_stride,
+                     const float* rs_ss_lo, int32_t rs_parts_lo, const float* rs_ss_hi, int32_t rs_parts_hi,
+                     int32_t rs_split_row, int32_t rs_ss_stride, float rs_inv_d, const float* rs_col_bias,
+                     int64_t rs_bias_step_stride, int32_t* block_n_out, void* stream);
+
+/* The first decoder layer's deferred-normalisation prep (no GEMM produced its stream): a_out bf16
+ * [rows, lda] = bf16(x * g), g at g + (*step) * g_step_stride; ss_out[row] = sum of x^2 over the
+ * row.  x f32 [rows, d], d = k * 128 <= 1024; step device int32.  Synchronises the stream. */
+int msd_op_prep_rows(const float* x, const float* g, int64_t g_step_stride, const int32_t* step, int32_t rows,
+                     int32_t d, void* a_out, int32_t lda, float* ss_out, void* stream);
+
+/* Host copies of the load-time conditioning tables (NULL skips one):
+ *   film      [num_steps][2 L][2 d]   FiLM scale | bias of each layer's two FiLM layers (j = 2l self,
+ *                                     2l + 1 mlp): the time MLP and FiLM dense of every step
+ *   gain      [num_steps][2 L][d]     gamma (1 + scale) of the same pre-norms
+ *   bias_qkv  [num_steps][L][3 hh]    FiLM bias of the self-attention pre-norm times the packed
+ *                                     bf16 QKV weights
+ *   bias_wi   [num_steps][L][2 F]     ... of the MLP pre-norm times the packed gated wi weights
+ *                                     (columns interleaved 32 of wi_0, 32 of wi_1)
+ * The last three exist with deferred normalisation only (bf16 mode); asking for them otherwise
+ * is refused (-1). */
+int msd_get_conditioning_tables(msd_ctx* ctx, float* film, float* gain, float* bias_qkv, float* bias_wi);
+
 /* LayerNorm (layers.py:632-649) followed by optional FiLM (layers.py:652-666) with explicit
  * scale|bias vector film [2*d] (NULL = none): out f32 (bf16-rounded) [rows, d]. */
 int msd_op_rmsnorm_film(const float* x, const float* gamma, const float* film, int32_t rows,

@@ -140,6 +140,13 @@ SYMBOLS = [
     ('msd_op_attention_view', ctypes.c_int,
      [_I, _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _I, _I, _I, _I, _I, _I,
       _P, _I, _I, _I, _P, ctypes.c_int64, _I, _P, _P, _I, _I, _P]),
+    ('msd_op_gemm_view', ctypes.c_int,
+     [_P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _I, _I, _I, _I, _I, _I,
+      _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _P, _I, _P, _I,
+      _P, _P, ctypes.c_int64, _P, ctypes.c_int64, _I, _P, _I, _P, _I,
+      _P, _I, _P, _I, _I, _I, ctypes.c_float, _P, ctypes.c_int64, ctypes.POINTER(_I), _P]),
+    ('msd_op_prep_rows', ctypes.c_int, [_P, _P, ctypes.c_int64, _P, _I, _I, _P, _I, _P, _P]),
+    ('msd_get_conditioning_tables', ctypes.c_int, [_P, _P, _P, _P, _P]),
     ('msd_op_audio_mel', ctypes.c_int, [_P, _I, ctypes.c_int64, _P, _P, _P, _P]),
     ('msd_op_audio_resample', ctypes.c_int,
      [_P, _I, ctypes.c_int64, _I, _I, _P, _I, _I, _P, _I, _P, ctypes.c_int64, _P]),

@@ -2040,6 +2040,83 @@ int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq
   return 0;
 }
 
+int msd_op_gemm_view(const void* a, int64_t a_off, int32_t lda, const void* b, int64_t b_off, int32_t ldb,
+                     int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n, int32_t variant,
+                     void* out, int64_t out_off, int32_t ldo, const float* resid, int64_t resid_off,
+                     const float* pos, int32_t pos_rows, const int32_t* pos_shift, int32_t dup_rows,
+                     const int32_t* step, const float* prep_g_lo, int64_t prep_g_lo_step_stride,
+                     const float* prep_g_hi, int64_t prep_g_hi_step_stride, int32_t prep_split_row,
+                     void* prep_a, int32_t prep_lda, float* prep_ss, int32_t prep_ss_stride,
+                     const float* rs_ss_lo, int32_t rs_parts_lo, const float* rs_ss_hi, int32_t rs_parts_hi,
+                     int32_t rs_split_row, int32_t rs_ss_stride, float rs_inv_d, const float* rs_col_bias,
+                     int64_t rs_bias_step_stride, int32_t* block_n_out, void* stream) {
+  MSD_REQUIRE(a && b && out, "msd_op_gemm_view: null argument");
+  MSD_REQUIRE(epilogue >= EPI_BF16 && epilogue <= EPI_RESID_PREP, "msd_op_gemm_view: unknown epilogue %d",
+              epilogue);
+  MSD_REQUIRE(a_off >= 0 && b_off >= 0 && out_off >= 0 && resid_off >= 0,
+              "msd_op_gemm_view: negative offset");
+  const bool f32_out = epilogue == EPI_F32 || epilogue == EPI_RESID_F32 || epilogue == EPI_POS_F32 ||
+                       epilogue == EPI_RESID_PREP;
+  GemmArgs g;
+  memset(&g, 0, sizeof(g));
+  g.A = static_cast<const bf16*>(a) + a_off; g.lda = lda;
+  g.B = static_cast<const bf16*>(b) + b_off; g.ldb = ldb;
+  g.M = M; g.N = N; g.K = K; g.epilogue = epilogue; g.block_n = block_n; g.variant = variant;
+  g.out = f32_out ? static_cast<void*>(static_cast<float*>(out) + out_off)
+                  : static_cast<void*>(static_cast<bf16*>(out) + out_off);
+  g.ldo = ldo;
+  g.resid = resid ? resid + resid_off : nullptr;
+  g.pos = pos; g.pos_rows = pos_rows; g.pos_shift = pos_shift; g.dup_rows = dup_rows;
+  g.step = step;
+  g.prep.g_lo = prep_g_lo; g.prep.g_lo_step_stride = prep_g_lo_step_stride;
+  g.prep.g_hi = prep_g_hi; g.prep.g_hi_step_stride = prep_g_hi_step_stride;
+  g.prep.split_row = prep_split_row;
+  g.prep.a = static_cast<bf16*>(prep_a); g.prep.lda = prep_lda;
+  g.prep.ss = prep_ss; g.prep.ss_stride = prep_ss_stride;
+  g.rs.ss_lo = rs_ss_lo; g.rs.parts_lo = rs_parts_lo; g.rs.ss_hi = rs_ss_hi; g.rs.parts_hi = rs_parts_hi;
+  g.rs.split_row = rs_split_row; g.rs.ss_stride = rs_ss_stride; g.rs.inv_d = rs_inv_d;
+  g.rs.col_bias = rs_col_bias; g.rs.bias_step_stride = rs_bias_step_stride;
+  MSD_REQUIRE(epilogue != EPI_RESID_PREP || g.prep.a != nullptr,
+              "msd_op_gemm_view: EPI_RESID_PREP needs prep_a");
+  MSD_REQUIRE(epilogue != EPI_POS_F32 || (pos != nullptr && pos_rows > 0),
+              "msd_op_gemm_view: EPI_POS_F32 needs pos / pos_rows");
+  const int bn = gemm_resolve_block_n(g);
+  MSD_REQUIRE(bn > 0, "msd_op_gemm_view: N=%d has no tile width (block_n %d, variant %d)", N, block_n, variant);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  g_pdl_skip_next = true;   // the operands were just written by the caller's own kernels
+  MSD_TRY(launch_gemm(g, st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  if (block_n_out) *block_n_out = bn;
+  return 0;
+}
+
+int msd_op_prep_rows(const float* x, const float* g, int64_t g_step_stride, const int32_t* step, int32_t rows,
+                     int32_t d, void* a_out, int32_t lda, float* ss_out, void* stream) {
+  MSD_REQUIRE(x && g && step && a_out && ss_out, "msd_op_prep_rows: null argument");
+  MSD_REQUIRE(rows > 0 && lda >= d && lda % 8 == 0, "msd_op_prep_rows: rows %d / lda %d (d %d)", rows, lda, d);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  g_pdl_skip_next = true;
+  MSD_TRY(launch_prep_rows(x, g, g_step_stride, step, rows, d, static_cast<bf16*>(a_out), lda, ss_out, st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int msd_get_conditioning_tables(msd_ctx* c, float* film, float* gain, float* bias_qkv, float* bias_wi) {
+  MSD_REQUIRE(c != nullptr, "msd_get_conditioning_tables: null context");
+  MSD_REQUIRE(c->weights_loaded, "msd_get_conditioning_tables: call msd_load_weights first");
+  MSD_REQUIRE(c->fused_norm || (!gain && !bias_qkv && !bias_wi),
+              "msd_get_conditioning_tables: deferred normalisation is off, there are no gain / bias tables");
+  const size_t steps = static_cast<size_t>(c->cfg.num_steps), Ld = static_cast<size_t>(c->cfg.num_decoder_layers);
+  const struct { float* dst; const float* src; size_t n; } tabs[4] = {
+      {film, c->film, steps * 2 * Ld * 2 * c->d},
+      {gain, c->gtab, steps * 2 * Ld * c->d},
+      {bias_qkv, c->btab_qkv, steps * Ld * 3 * c->hh},
+      {bias_wi, c->btab_wi, steps * Ld * 2 * c->F}};
+  for (const auto& t : tabs)
+    if (t.dst) MSD_CUDA_CHECK(cudaMemcpy(t.dst, t.src, t.n * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 int msd_op_rmsnorm_film(const float* x, const float* gamma, const float* film, int32_t rows,
                         int32_t d, float* out, void* stream) {
   MSD_REQUIRE(x && gamma && out, "msd_op_rmsnorm_film: null argument");

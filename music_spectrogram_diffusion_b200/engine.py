@@ -232,6 +232,21 @@ class Engine:
     _native.check(self.lib.msd_get_step_table(self._h, tab.ctypes.data), 'msd_get_step_table')
     return tab
 
+  def conditioning_tables(self, deferred: bool = True) -> Dict[str, np.ndarray]:
+    """The load-time conditioning tables (msd_get_conditioning_tables), float32:
+    film [steps, 2 L, 2 d] and, with deferred=True (bf16 mode), gain [steps, 2 L, d],
+    bias_qkv [steps, L, 3 hh] and bias_wi [steps, L, 2 F]."""
+    c = self.cfg
+    s, L, d, hh = c.num_steps, c.num_decoder_layers, c.emb_dim, c.num_heads * c.head_dim
+    shapes = dict(film=(s, 2 * L, 2 * d))
+    if deferred:
+      shapes.update(gain=(s, 2 * L, d), bias_qkv=(s, L, 3 * hh), bias_wi=(s, L, 2 * c.mlp_dim))
+    out = {k: np.zeros(v, dtype=np.float32) for k, v in shapes.items()}
+    ptrs = [ctypes.c_void_p(out[k].ctypes.data) if k in out else None
+            for k in ('film', 'gain', 'bias_qkv', 'bias_wi')]
+    _native.check(self.lib.msd_get_conditioning_tables(self._h, *ptrs), 'msd_get_conditioning_tables')
+    return out
+
 
 def launch_count() -> int:
   return int(_native.load().msd_launch_count())
@@ -409,6 +424,149 @@ def op_attention_view(q: torch.Tensor, q_off: int, ldq: int, k: torch.Tensor, k_
       acc, _ptr(q), q_off, ldq, _ptr(k), k_off, ldk, _ptr(v), v_off, ldv, nb, heads, lq, lk,
       kv_batch_rows, kv_row0, _ptr(key_mask), mask_len, mask_word0, int(kv_static), _ptr(out), o_col,
       o_ld, _ptr(part_o), _ptr(part_ml), splits, tail, _stream(q.device)), 'msd_op_attention_view')
+
+
+GEMM_EPILOGUES = dict(EPILOGUES, f32=1, resid_prep=6)
+_F32_OUT = ('f32', 'resid_f32', 'pos_f32', 'resid_prep')
+
+
+def _check_dev(name: str, t: torch.Tensor, dtype: torch.dtype, device: torch.device) -> None:
+  if t.dtype != dtype or t.device != device:
+    raise ValueError(f'{name}: expected a {dtype} tensor on {device}, got {t.dtype} on {t.device}')
+
+
+def _check_vector(name: str, t: torch.Tensor, off: int, n: int, device: torch.device) -> None:
+  """n float32 values of t from element `off`."""
+  _check_dev(name, t, torch.float32, device)
+  _check_view(name, t, off, off + n, 1, n, 4)
+
+
+def _step_value(step: Optional[torch.Tensor], device: torch.device) -> int:
+  """The device step index a launch will read (0 without one)."""
+  if step is None:
+    return 0
+  _check_dev('step', step, torch.int32, device)
+  if step.numel() != 1:
+    raise ValueError('step: expected one int32 element')
+  s = int(step.item())
+  if s < 0:
+    raise ValueError(f'step: {s} is negative')
+  return s
+
+
+def op_gemm_view(a: torch.Tensor, a_off: int, lda: int, b: torch.Tensor, b_off: int, ldb: int,
+                 m: int, n: int, k: int, epilogue: str, out: torch.Tensor, out_off: int, ldo: int,
+                 block_n: int = 0, variant: int = 0, resid: Optional[torch.Tensor] = None,
+                 resid_off: int = 0, pos: Optional[torch.Tensor] = None,
+                 pos_shift: Optional[torch.Tensor] = None, dup_rows: int = 0,
+                 step: Optional[torch.Tensor] = None, prep: Optional[dict] = None,
+                 rs: Optional[dict] = None) -> int:
+  """The GEMM over views of caller-owned device buffers, with every argument the engine's decoder
+  sets (msd_op_gemm_view); returns the tile width that ran.  a / b: bf16, out = a[m, k] b[n, k]^T
+  through `epilogue` (GEMM_EPILOGUES) into out (f32 or bf16 by epilogue) at out_off / ldo.
+  prep (epilogue 'resid_prep'): dict(g_lo=(t, off, step_stride), g_hi=(t, off, step_stride),
+  split_row, a, lda, ss, ss_stride).  rs (row scale on 'bf16' / 'gated_gelu'): dict(ss_lo, parts_lo,
+  ss_hi, parts_hi, split_row, ss_stride, inv_d, bias=(t, off, step_stride) or None).
+  Every view is checked to lie inside its tensor before the library is called; step-indexed
+  vectors at the step `step` holds, prep.ss for the narrowest tile the launch may run (N / 64
+  partial sums, or N / block_n)."""
+  if epilogue not in GEMM_EPILOGUES:
+    raise ValueError(f'unknown epilogue {epilogue!r} (expected one of {sorted(GEMM_EPILOGUES)})')
+  dev = a.device
+  if m <= 0 or n <= 0 or k <= 0 or m % 128 or k % 64:
+    raise ValueError(f'm={m}, n={n}, k={k}: m must be a positive multiple of 128, k of 64')
+  for name, t in (('a', a), ('b', b)):
+    _check_dev(name, t, torch.bfloat16, dev)
+  _check_view('a', a, a_off, lda, m, k, 2)
+  _check_view('b', b, b_off, ldb, n, k, 2)
+  f32_out = epilogue in _F32_OUT
+  _check_dev('out', out, torch.float32 if f32_out else torch.bfloat16, dev)
+  cols = {'gated_gelu': n // 2, 'gated_gelu_split3': 3 * (n // 2)}.get(epilogue, n)
+  _check_view('out', out, out_off, ldo, m + (dup_rows if epilogue == 'pos_f32' else 0), cols,
+              4 if f32_out else 2)
+  if resid is not None:
+    _check_dev('resid', resid, torch.float32, dev)
+    _check_view('resid', resid, resid_off, ldo, m, n, 4)
+  elif epilogue in ('resid_f32', 'resid_prep'):
+    raise ValueError(f'epilogue {epilogue!r} needs resid')
+  pos_rows = 0
+  if epilogue == 'pos_f32':
+    if pos is None:
+      raise ValueError("epilogue 'pos_f32' needs pos")
+    _check_dev('pos', pos, torch.float32, dev)
+    pos_rows = pos.shape[0]
+    _check_view('pos', pos, 0, n, pos_rows, n, 4)
+    if pos_shift is not None:
+      _check_dev('pos_shift', pos_shift, torch.int32, dev)
+      if pos_shift.numel() < -(-m // pos_rows):
+        raise ValueError(f'pos_shift: {pos_shift.numel()} entries for {-(-m // pos_rows)} sequences')
+  s = _step_value(step, dev)
+  pa = dict(g_lo=None, g_lo_s=0, g_hi=None, g_hi_s=0, split_row=0, a=None, lda=0, ss=None, ss_stride=0)
+  if prep is not None:
+    if epilogue != 'resid_prep':
+      raise ValueError('prep goes with the resid_prep epilogue')
+    for key in ('g_lo', 'g_hi'):
+      t, off, stride = prep[key]
+      if stride and step is None:
+        raise ValueError(f'prep.{key}: a step stride needs the device step')
+      _check_vector(f'prep.{key}', t, off + s * stride, n, dev)
+      pa[key] = ctypes.c_void_p(t.data_ptr() + 4 * off)
+      pa[key + '_s'] = stride
+    _check_dev('prep.a', prep['a'], torch.bfloat16, dev)
+    _check_view('prep.a', prep['a'], 0, prep['lda'], m, n, 2)
+    _check_dev('prep.ss', prep['ss'], torch.float32, dev)
+    if prep['ss_stride'] < m:
+      raise ValueError(f'prep.ss_stride {prep["ss_stride"]} < m = {m}')
+    _check_view('prep.ss', prep['ss'], 0, prep['ss_stride'], n // (block_n or 64), m, 4)
+    pa.update(split_row=prep['split_row'], a=_ptr(prep['a']), lda=prep['lda'], ss=_ptr(prep['ss']),
+              ss_stride=prep['ss_stride'])
+  elif epilogue == 'resid_prep':
+    raise ValueError("epilogue 'resid_prep' needs prep")
+  ra = dict(ss_lo=None, parts_lo=0, ss_hi=None, parts_hi=0, split_row=0, ss_stride=0, inv_d=0.0,
+            bias=None, bias_s=0)
+  if rs is not None:
+    if epilogue not in ('bf16', 'gated_gelu'):
+      raise ValueError('the row scale goes with the bf16 and gated_gelu epilogues')
+    for key in ('lo', 'hi'):
+      t, parts = rs['ss_' + key], rs['parts_' + key]
+      _check_dev(f'rs.ss_{key}', t, torch.float32, dev)
+      if parts <= 0 or rs['ss_stride'] < m:
+        raise ValueError(f'rs: parts_{key} = {parts} / ss_stride {rs["ss_stride"]} (m = {m})')
+      _check_view(f'rs.ss_{key}', t, 0, rs['ss_stride'], parts, m, 4)
+      ra['ss_' + key], ra['parts_' + key] = _ptr(t), parts
+    ra.update(split_row=rs['split_row'], ss_stride=rs['ss_stride'], inv_d=rs['inv_d'])
+    if rs.get('bias') is not None:
+      t, off, stride = rs['bias']
+      if stride and step is None:
+        raise ValueError('rs.bias: a step stride needs the device step')
+      _check_vector('rs.bias', t, off + s * stride, n, dev)
+      ra['bias'], ra['bias_s'] = ctypes.c_void_p(t.data_ptr() + 4 * off), stride
+  bn = ctypes.c_int32(0)
+  _native.check(_native.load().msd_op_gemm_view(
+      _ptr(a), a_off, lda, _ptr(b), b_off, ldb, m, n, k, GEMM_EPILOGUES[epilogue], block_n, variant,
+      _ptr(out), out_off, ldo, _ptr(resid), resid_off, _ptr(pos), pos_rows, _ptr(pos_shift), dup_rows,
+      _ptr(step), pa['g_lo'], pa['g_lo_s'], pa['g_hi'], pa['g_hi_s'], pa['split_row'], pa['a'], pa['lda'],
+      pa['ss'], pa['ss_stride'], ra['ss_lo'], ra['parts_lo'], ra['ss_hi'], ra['parts_hi'],
+      ra['split_row'], ra['ss_stride'], ra['inv_d'], ra['bias'], ra['bias_s'], ctypes.byref(bn),
+      _stream(dev)), 'msd_op_gemm_view')
+  return bn.value
+
+
+def op_prep_rows(x: torch.Tensor, g: torch.Tensor, g_off: int, g_step_stride: int, step: torch.Tensor,
+                 rows: int, d: int, a_out: torch.Tensor, lda: int, ss_out: torch.Tensor) -> None:
+  """The first decoder layer's prep (msd_op_prep_rows): a_out [rows, lda] bf16 = bf16(x * g_step),
+  ss_out[:rows] = row sums of x^2; x f32 rows of d, g_step the d gains at g_off + step *
+  g_step_stride.  Views are checked before the library is called."""
+  dev = x.device
+  _check_dev('x', x, torch.float32, dev)
+  _check_view('x', x, 0, d, rows, d, 4)
+  _check_vector('g', g, g_off + _step_value(step, dev) * g_step_stride, d, dev)
+  _check_dev('a_out', a_out, torch.bfloat16, dev)
+  _check_view('a_out', a_out, 0, lda, rows, d, 2)
+  _check_vector('ss_out', ss_out, 0, rows, dev)
+  _native.check(_native.load().msd_op_prep_rows(
+      _ptr(x), ctypes.c_void_p(g.data_ptr() + 4 * g_off), g_step_stride, _ptr(step), rows, d,
+      _ptr(a_out), lda, _ptr(ss_out), _stream(dev)), 'msd_op_prep_rows')
 
 
 def op_jax_bits(seed: int, step: int, n: int, device: torch.device) -> torch.Tensor:
