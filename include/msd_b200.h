@@ -160,6 +160,10 @@ int msd_get_encodings(msd_ctx* ctx, float* enc_out, void* stream);
  * (predict_eps_from_x0 at logsnr_t: eps = e1 (z - x0 e2)), 14 logsnr_train, 15 reserved. */
 int msd_get_step_table(msd_ctx* ctx, float* table_host);
 
+/* The same table for a configuration, without a context or a GPU: validates cfg as msd_create does
+ * (-1 when it would refuse it), then writes table_host [cfg->num_steps][16] (host). */
+int msd_step_table(const msd_config* cfg, float* table_host);
+
 /* Profiling hook: runs diffusion step `step_i` (1 <= step_i < num_steps) of the batch of the
  * last msd_encode `reps` times WITHOUT graph capture, bracketing every kernel launch with CUDA
  * events on the launching stream.  out[5][4] (doubles), one row per kernel class
@@ -317,6 +321,46 @@ int msd_op_prep_rows(const float* x, const float* g, int64_t g_step_stride, cons
  * The last three exist with deferred normalisation only (bf16 mode); asking for them otherwise
  * is refused (-1). */
 int msd_get_conditioning_tables(msd_ctx* ctx, float* film, float* gain, float* bias_qkv, float* bias_wi);
+
+/* The sampler kernel (one reverse step: guidance combine, x0, clip, DDPM / DDIM update, noise) on
+ * caller-owned device buffers, with the fields the engine sets (no guidance split, no prefetch):
+ *   eps       f32 [passes * n]: the model output of the conditional pass, then the unconditional one
+ *   z         f32 [n], updated in place; z_split bf16 [n / n_dims, 3 n_dims] = [hi | lo | hi] of new z
+ *   mel_out   f32 [n] or NULL: scale_to_features(z) written at step 0 only
+ *   noise     f32 [num_steps, n] (row i read at step i) or NULL: generated from seed (rng_kind 0,
+ *             Philox stream i + 1) or rng_keys [num_steps + 1][2] (rng_kind 1, row i + 1)
+ *   coef      f32 [num_steps, 16] (msd_get_step_table layout)
+ *   per_row   generated noise of row b = idx / n_row from row_seeds[b] (uint64, rng_kind 0) or
+ *             row_keys + b * row_key_stride (rng_kind 1): n_row % 8 == 0, n < 2^32
+ * step != NULL: the step index is read from that device int32 (one launch, per_row 0).
+ * step == NULL: the graph's path.  A device RunArgs {noise, mel_out, seed, step = run_step, per_row}
+ * is built, the kernel runs `launches` times behind each other (each launch advances the step), and
+ * run_out[0] / run_out[1] (host) receive the RunArgs step and done counter found afterwards.
+ * Refused (-1): null z / z_split / eps / coef, n not a positive multiple of n_dims (both multiples of
+ * 4), passes other than 1 or 2, the jax stream without keys or with n % 8 != 0 or n >= 2^32, per-row
+ * streams without their table or with n_row % 8 != 0 or n >= 2^32, and steps outside the table.
+ * Synchronises the stream. */
+int msd_op_sampler_step(const float* eps, float* z, void* z_split, float* mel_out, const float* noise,
+                        const float* coef, int32_t num_steps, const int32_t* step, int64_t n, int32_t n_dims,
+                        int32_t passes, float cond_weight, int32_t clip_x0, int32_t ddim, float feat_min,
+                        float feat_max, uint64_t seed, int32_t rng_kind, const uint32_t* rng_keys,
+                        int64_t n_row, const uint32_t* row_keys, int64_t row_key_stride,
+                        const uint64_t* row_seeds, int32_t run_step, int32_t per_row, int32_t launches,
+                        int32_t* run_out, void* stream);
+
+/* The sampler's initial state: z f32 [n] = init_z (device copy) or, with init_z NULL, the draw of
+ * Philox stream 0 of seed (rng_kind 0) or of key rng_keys[0..1] (rng_kind 1); n_row > 0: row b's own
+ * draw from row_seeds[b] / rng_keys + b * row_key_stride.  z_split as in msd_op_sampler_step.
+ * Synchronises the stream. */
+int msd_op_init_z(const float* init_z, float* z, void* z_split, int64_t n, int32_t n_dims, uint64_t seed,
+                  int32_t rng_kind, const uint32_t* rng_keys, int64_t n_row, int64_t row_key_stride,
+                  const uint64_t* row_seeds, void* stream);
+
+/* The encoder's context-feature front end (scale_features(clip=True), audio_codecs.py:166-174):
+ * feat f32 [rows, n_dims] -> out_split bf16 [rows, 3 n_dims] = [hi | lo | hi] of
+ * 2 (clip(f, feat_min, feat_max) - feat_min) / (feat_max - feat_min) - 1.  Synchronises the stream. */
+int msd_op_scale_split(const float* feat, void* out_split, int64_t rows, int32_t n_dims, float feat_min,
+                       float feat_max, void* stream);
 
 /* LayerNorm (layers.py:632-649) followed by optional FiLM (layers.py:652-666) with explicit
  * scale|bias vector film [2*d] (NULL = none): out f32 (bf16-rounded) [rows, d]. */

@@ -123,6 +123,7 @@ SYMBOLS = [
     ('msd_decode_eps', ctypes.c_int, [_P, _P, _I, _I, _P, _P]),
     ('msd_get_encodings', ctypes.c_int, [_P, _P, _P]),
     ('msd_get_step_table', ctypes.c_int, [_P, _P]),
+    ('msd_step_table', ctypes.c_int, [ctypes.POINTER(MsdConfig), _P]),
     ('msd_profile_step', ctypes.c_int, [_P, _I, _I, _P]),
     ('msd_launch_count', ctypes.c_uint64, []),
     ('msd_op_dense', ctypes.c_int, [_P, _P, _I, _I, _I, _P, _P]),
@@ -147,6 +148,14 @@ SYMBOLS = [
       _P, _I, _P, _I, _I, _I, ctypes.c_float, _P, ctypes.c_int64, ctypes.POINTER(_I), _P]),
     ('msd_op_prep_rows', ctypes.c_int, [_P, _P, ctypes.c_int64, _P, _I, _I, _P, _I, _P, _P]),
     ('msd_get_conditioning_tables', ctypes.c_int, [_P, _P, _P, _P, _P]),
+    ('msd_op_sampler_step', ctypes.c_int,
+     [_P, _P, _P, _P, _P, _P, _I, _P, ctypes.c_int64, _I, _I, ctypes.c_float, _I, _I, ctypes.c_float,
+      ctypes.c_float, ctypes.c_uint64, _I, _P, ctypes.c_int64, _P, ctypes.c_int64, _P, _I, _I, _I,
+      ctypes.POINTER(_I), _P]),
+    ('msd_op_init_z', ctypes.c_int,
+     [_P, _P, _P, ctypes.c_int64, _I, ctypes.c_uint64, _I, _P, ctypes.c_int64, ctypes.c_int64, _P, _P]),
+    ('msd_op_scale_split', ctypes.c_int,
+     [_P, _P, ctypes.c_int64, _I, ctypes.c_float, ctypes.c_float, _P]),
     ('msd_op_audio_mel', ctypes.c_int, [_P, _I, ctypes.c_int64, _P, _P, _P, _P]),
     ('msd_op_audio_resample', ctypes.c_int,
      [_P, _I, ctypes.c_int64, _I, _I, _P, _I, _I, _P, _I, _P, ctypes.c_int64, _P]),

@@ -184,6 +184,12 @@ __device__ __forceinline__ float4 philox_normal4(unsigned long long seed, uint32
   return make_float4(ra * ca, ra * sa, rb * cb, rb * sb);
 }
 
+// clip(v, lo, hi) as jnp.clip and torch.clamp compute it: a NaN stays NaN (fminf / fmaxf alone
+// return the non-NaN operand, which would turn a NaN into a plausible bound)
+__device__ __forceinline__ float clip_nan(float v, float lo, float hi) {
+  return v != v ? v : fminf(fmaxf(v, lo), hi);
+}
+
 __device__ __forceinline__ void store_split4(bf16* zs, long long idx, int n_dims, float4 v) {
   const long long row = idx / n_dims;
   const int col = static_cast<int>(idx - row * n_dims);
@@ -324,8 +330,8 @@ __device__ __forceinline__ void sampler_step_body(const SamplerArgs& a, int step
     x0.z = fmaf(q1, mo.z, q0 * z.z); x0.w = fmaf(q1, mo.w, q0 * z.w);
   }
   if (a.clip_x0) {
-    x0.x = fminf(fmaxf(x0.x, -1.f), 1.f); x0.y = fminf(fmaxf(x0.y, -1.f), 1.f);
-    x0.z = fminf(fmaxf(x0.z, -1.f), 1.f); x0.w = fminf(fmaxf(x0.w, -1.f), 1.f);
+    x0.x = clip_nan(x0.x, -1.f, 1.f); x0.y = clip_nan(x0.y, -1.f, 1.f);
+    x0.z = clip_nan(x0.z, -1.f, 1.f); x0.w = clip_nan(x0.w, -1.f, 1.f);
     if (a.ddim) {  // pred_eps = predict_eps_from_x0(z, clipped x0, logsnr_t) (437-439)
       e.x = e1 * (z.x - x0.x * e2); e.y = e1 * (z.y - x0.y * e2);
       e.z = e1 * (z.z - x0.z * e2); e.w = e1 * (z.w - x0.w * e2);
@@ -517,10 +523,10 @@ scale_split_kernel(const float* feat, bf16* out, long long n, int n_dims, float 
   float4 f = *reinterpret_cast<const float4*>(feat + idx);
   // scale_features(clip=True), msd/audio_codecs.py:166-174 with output_range (-1, 1)
   const float inv = 1.0f / (fmax - fmin);
-  f.x = (fminf(fmaxf(f.x, fmin), fmax) - fmin) * inv * 2.0f - 1.0f;
-  f.y = (fminf(fmaxf(f.y, fmin), fmax) - fmin) * inv * 2.0f - 1.0f;
-  f.z = (fminf(fmaxf(f.z, fmin), fmax) - fmin) * inv * 2.0f - 1.0f;
-  f.w = (fminf(fmaxf(f.w, fmin), fmax) - fmin) * inv * 2.0f - 1.0f;
+  f.x = (clip_nan(f.x, fmin, fmax) - fmin) * inv * 2.0f - 1.0f;
+  f.y = (clip_nan(f.y, fmin, fmax) - fmin) * inv * 2.0f - 1.0f;
+  f.z = (clip_nan(f.z, fmin, fmax) - fmin) * inv * 2.0f - 1.0f;
+  f.w = (clip_nan(f.w, fmin, fmax) - fmin) * inv * 2.0f - 1.0f;
   store_split4(out, idx, n_dims, f);
 }
 

@@ -1339,6 +1339,15 @@ int msd_get_step_table(msd_ctx* c, float* table_host) {
   return 0;
 }
 
+int msd_step_table(const msd_config* cfg, float* table_host) {
+  MSD_REQUIRE(cfg && table_host, "msd_step_table: null argument");
+  MSD_TRY(validate(cfg));
+  std::vector<float> tab;
+  build_step_table(*cfg, tab);
+  memcpy(table_host, tab.data(), tab.size() * sizeof(float));
+  return 0;
+}
+
 int msd_decode_eps(msd_ctx* c, const float* z, int32_t step_i, int32_t conditioned, float* eps_out,
                    void* stream) {
   MSD_REQUIRE(c && z && eps_out, "msd_decode_eps: null argument");
@@ -2097,6 +2106,91 @@ int msd_op_prep_rows(const float* x, const float* g, int64_t g_step_stride, cons
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   g_pdl_skip_next = true;
   MSD_TRY(launch_prep_rows(x, g, g_step_stride, step, rows, d, static_cast<bf16*>(a_out), lda, ss_out, st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int msd_op_sampler_step(const float* eps, float* z, void* z_split, float* mel_out, const float* noise,
+                        const float* coef, int32_t num_steps, const int32_t* step, int64_t n, int32_t n_dims,
+                        int32_t passes, float cond_weight, int32_t clip_x0, int32_t ddim, float feat_min,
+                        float feat_max, uint64_t seed, int32_t rng_kind, const uint32_t* rng_keys,
+                        int64_t n_row, const uint32_t* row_keys, int64_t row_key_stride,
+                        const uint64_t* row_seeds, int32_t run_step, int32_t per_row, int32_t launches,
+                        int32_t* run_out, void* stream) {
+  MSD_REQUIRE(eps && z && z_split && coef, "msd_op_sampler_step: null argument");
+  MSD_REQUIRE(n > 0 && n_dims > 0 && n % 4 == 0 && n_dims % 4 == 0 && n % n_dims == 0 && num_steps > 0,
+              "msd_op_sampler_step: n=%lld must be a positive multiple of n_dims=%d, both multiples of 4",
+              static_cast<long long>(n), n_dims);
+  MSD_REQUIRE(passes == 1 || passes == 2, "msd_op_sampler_step: passes must be 1 or 2 (got %d)", passes);
+  MSD_REQUIRE(rng_kind == 0 || rng_kind == 1, "msd_op_sampler_step: rng_kind must be 0 or 1");
+  MSD_REQUIRE(rng_kind == 0 || per_row || (rng_keys != nullptr && n % 8 == 0 && n < (1ll << 32)),
+              "msd_op_sampler_step: the jax stream needs its key table and a draw of k*8 < 2^32 elements");
+  MSD_REQUIRE(!per_row || (n_row > 0 && n_row % 8 == 0 && n % n_row == 0 && n < (1ll << 32) &&
+                           (rng_kind == 0 ? row_seeds != nullptr : row_keys != nullptr)),
+              "msd_op_sampler_step: per-row streams need rows of k*8 elements, n < 2^32 and the row table");
+  MSD_REQUIRE(step == nullptr || (!per_row && launches == 1),
+              "msd_op_sampler_step: per-row streams and several launches need the RunArgs path (step NULL)");
+  MSD_REQUIRE(step != nullptr || run_out != nullptr, "msd_op_sampler_step: the RunArgs path needs run_out");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int first = run_step;
+  if (step != nullptr) MSD_CUDA_CHECK(cudaMemcpy(&first, step, sizeof(int), cudaMemcpyDeviceToHost));
+  MSD_REQUIRE(launches >= 1 && first < num_steps && first - launches + 1 >= 0,
+              "msd_op_sampler_step: %d launch(es) from step %d leave the table of %d steps", launches, first,
+              num_steps);
+  SamplerArgs a;
+  memset(&a, 0, sizeof(a));
+  a.eps = eps; a.z = z; a.z_split = static_cast<bf16*>(z_split); a.coef = coef;
+  a.n = n; a.n_dims = n_dims; a.passes = passes; a.cond_weight = cond_weight;
+  a.clip_x0 = clip_x0; a.ddim = ddim; a.feat_min = feat_min; a.feat_max = feat_max;
+  a.rng_kind = rng_kind; a.rng_keys = rng_keys;
+  a.n_row = n_row; a.row_keys = row_keys; a.row_key_stride = row_key_stride;
+  a.row_seeds = reinterpret_cast<const unsigned long long*>(row_seeds);
+  TempBufs tb;
+  if (step != nullptr) {
+    a.step = step; a.noise = noise; a.mel_out = mel_out; a.seed = seed;
+    g_pdl_skip_next = true;   // the inputs were just written by the caller's own kernels
+    MSD_TRY(launch_sampler_step(a, st));
+    MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  RunArgs ra;
+  memset(&ra, 0, sizeof(ra));
+  ra.noise = noise; ra.mel_out = mel_out; ra.seed = seed; ra.step = run_step; ra.per_row = per_row;
+  MSD_TRY(tb.get(&a.run, 1));
+  MSD_CUDA_CHECK(cudaMemcpyAsync(a.run, &ra, sizeof(ra), cudaMemcpyHostToDevice, st));
+  // the first launch follows the upload; the next ones are PDL launches behind the previous step's
+  // sampler kernel, which is what the step graph's first kernel sees
+  g_pdl_skip_next = true;
+  for (int i = 0; i < launches; ++i) MSD_TRY(launch_sampler_step(a, st));
+  MSD_CUDA_CHECK(cudaMemcpyAsync(&ra, a.run, sizeof(ra), cudaMemcpyDeviceToHost, st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  run_out[0] = ra.step;
+  run_out[1] = static_cast<int32_t>(ra.done);
+  return 0;
+}
+
+int msd_op_init_z(const float* init_z, float* z, void* z_split, int64_t n, int32_t n_dims, uint64_t seed,
+                  int32_t rng_kind, const uint32_t* rng_keys, int64_t n_row, int64_t row_key_stride,
+                  const uint64_t* row_seeds, void* stream) {
+  MSD_REQUIRE(z && z_split, "msd_op_init_z: null argument");
+  MSD_REQUIRE(n > 0 && n_dims > 0 && n % 4 == 0 && n_dims % 4 == 0 && n % n_dims == 0,
+              "msd_op_init_z: n=%lld must be a positive multiple of n_dims=%d, both multiples of 4",
+              static_cast<long long>(n), n_dims);
+  MSD_REQUIRE(rng_kind == 0 || rng_kind == 1, "msd_op_init_z: rng_kind must be 0 or 1");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  MSD_TRY(launch_init_z(init_z, z, static_cast<bf16*>(z_split), n, n_dims, seed, st, rng_kind, rng_keys, n_row,
+                        row_key_stride, reinterpret_cast<const unsigned long long*>(row_seeds)));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int msd_op_scale_split(const float* feat, void* out_split, int64_t rows, int32_t n_dims, float feat_min,
+                       float feat_max, void* stream) {
+  MSD_REQUIRE(feat && out_split, "msd_op_scale_split: null argument");
+  MSD_REQUIRE(rows > 0 && n_dims > 0 && n_dims % 4 == 0, "msd_op_scale_split: rows %lld / n_dims %d",
+              static_cast<long long>(rows), n_dims);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  MSD_TRY(launch_scale_split(feat, static_cast<bf16*>(out_split), rows, n_dims, feat_min, feat_max, st));
   MSD_CUDA_CHECK(cudaStreamSynchronize(st));
   return 0;
 }

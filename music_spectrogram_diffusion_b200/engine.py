@@ -569,6 +569,155 @@ def op_prep_rows(x: torch.Tensor, g: torch.Tensor, g_off: int, g_step_stride: in
       _ptr(a_out), lda, _ptr(ss_out), _stream(dev)), 'msd_op_prep_rows')
 
 
+STEP_COLS = 16   # floats per diffusion step in the sampler table (msd_get_step_table)
+
+
+def step_table_for(cfg: _native.MsdConfig) -> np.ndarray:
+  """The sampler's per-step table [num_steps, STEP_COLS] float32 for cfg (msd_step_table): what
+  Engine.step_table() returns for a context created from cfg, computed on the host without a GPU."""
+  if not isinstance(cfg, _native.MsdConfig):
+    raise TypeError(f'cfg: expected an MsdConfig, got {type(cfg).__name__}')
+  if cfg.num_steps <= 0:
+    raise ValueError(f'num_steps = {cfg.num_steps} must be positive')
+  tab = np.zeros((cfg.num_steps, STEP_COLS), dtype=np.float32)
+  _native.check(_native.load().msd_step_table(ctypes.byref(cfg), tab.ctypes.data), 'msd_step_table')
+  return tab
+
+
+def _check_flat(name: str, t: torch.Tensor, dtype: torch.dtype, device: torch.device, n: int) -> None:
+  """t is a contiguous `dtype` tensor on `device` with at least n elements."""
+  _check_dev(name, t, dtype, device)
+  if not t.is_contiguous():
+    raise ValueError(f'{name}: tensor must be contiguous')
+  if t.numel() < n:
+    raise ValueError(f'{name}: {t.numel()} elements, the launch reads or writes {n}')
+
+
+def _check_state(z: torch.Tensor, z_split: torch.Tensor, n: int, n_dims: int) -> None:
+  if n <= 0 or n_dims <= 0 or n % 4 or n_dims % 4 or n % n_dims:
+    raise ValueError(f'n = {n} must be a positive multiple of n_dims = {n_dims}, both multiples of 4')
+  if not z.is_cuda:
+    raise ValueError(f'z: expected a CUDA tensor, got one on {z.device}')
+  _check_flat('z', z, torch.float32, z.device, n)
+  _check_flat('z_split', z_split, torch.bfloat16, z.device, 3 * n)
+
+
+def _check_streams(n: int, steps: int, rng_kind: int, rng_keys: Optional[torch.Tensor], n_row: int,
+                   row_keys: Optional[torch.Tensor], row_key_stride: int,
+                   row_seeds: Optional[torch.Tensor], per_row: bool, device: torch.device) -> None:
+  """The key / seed tables a generated draw of n elements reads: rng_kind 1 reads key rows
+  0 .. steps of rng_keys (int32 storage of uint32 words, 2 per row); per-row streams read row b's
+  table at row_keys + b * row_key_stride, or its Philox seed row_seeds[b] (int64 storage)."""
+  if rng_kind not in (0, 1):
+    raise ValueError(f'rng_kind = {rng_kind} must be 0 (philox) or 1 (jax)')
+  if not per_row:
+    if rng_kind == 1:
+      if rng_keys is None or n % 8 or n >= 1 << 32:
+        raise ValueError('the jax stream needs rng_keys and a draw of k * 8 < 2^32 elements')
+      _check_flat('rng_keys', rng_keys, torch.int32, device, 2 * (steps + 1))
+    return
+  if n_row <= 0 or n_row % 8 or n % n_row or n >= 1 << 32:
+    raise ValueError(f'per-row streams: n_row = {n_row} must be a multiple of 8 dividing n = {n} < 2^32')
+  rows = n // n_row
+  if rng_kind == 1:
+    if row_keys is None or row_key_stride < 2 * (steps + 1):
+      raise ValueError(f'per-row jax streams need row_keys with a stride >= {2 * (steps + 1)}')
+    _check_flat('row_keys', row_keys, torch.int32, device, (rows - 1) * row_key_stride + 2 * (steps + 1))
+  else:
+    if row_seeds is None:
+      raise ValueError('per-row Philox streams need row_seeds')
+    _check_flat('row_seeds', row_seeds, torch.int64, device, rows)
+
+
+def op_sampler_step(eps: torch.Tensor, z: torch.Tensor, z_split: torch.Tensor, coef: torch.Tensor,
+                    n: int, passes: int, cond_weight: float, clip_x0: bool, ddim: bool,
+                    feat_min: float, feat_max: float, n_dims: int = 128,
+                    step: Optional[torch.Tensor] = None, run_step: Optional[int] = None,
+                    launches: int = 1, mel_out: Optional[torch.Tensor] = None,
+                    noise: Optional[torch.Tensor] = None, seed: int = 0, rng_kind: int = 0,
+                    rng_keys: Optional[torch.Tensor] = None, per_row: bool = False, n_row: int = 0,
+                    row_keys: Optional[torch.Tensor] = None, row_key_stride: int = 0,
+                    row_seeds: Optional[torch.Tensor] = None):
+  """The sampler kernel on caller-owned device buffers (msd_op_sampler_step): updates z[:n] and
+  z_split[:3 n] in place (and mel_out[:n] at step 0).  eps f32 [passes * n], coef f32 [steps, 16],
+  noise f32 [steps, n] or None (generated: seed / rng_keys, or the per-row tables).
+  Exactly one of `step` (device int32: one launch, the step read from there) and `run_step` (the
+  graph's RunArgs path: `launches` launches from that step) is given; the latter returns the
+  (step, done) the RunArgs hold afterwards.  Every buffer is checked before the library is called."""
+  if (step is None) == (run_step is None):
+    raise ValueError('give exactly one of step (device) and run_step (RunArgs path)')
+  if passes not in (1, 2):
+    raise ValueError(f'passes = {passes} must be 1 or 2')
+  _check_state(z, z_split, n, n_dims)
+  dev = z.device
+  _check_flat('eps', eps, torch.float32, dev, passes * n)
+  _check_dev('coef', coef, torch.float32, dev)
+  if coef.dim() != 2 or coef.shape[1] != STEP_COLS or coef.shape[0] <= 0 or not coef.is_contiguous():
+    raise ValueError(f'coef: expected a contiguous [num_steps, {STEP_COLS}] table, got {tuple(coef.shape)}')
+  steps = coef.shape[0]
+  if step is not None:
+    first = _step_value(step, dev)
+    if per_row or launches != 1:
+      raise ValueError('per-row streams and several launches take the RunArgs path (run_step)')
+  else:
+    first = int(run_step)
+  if launches < 1 or first >= steps or first - launches + 1 < 0:
+    raise ValueError(f'{launches} launch(es) from step {first} leave the table of {steps} steps')
+  if mel_out is not None:
+    _check_flat('mel_out', mel_out, torch.float32, dev, n)
+  if noise is not None:
+    _check_flat('noise', noise, torch.float32, dev, steps * n)
+  else:
+    _check_streams(n, steps, rng_kind, rng_keys, n_row, row_keys, row_key_stride, row_seeds, per_row, dev)
+  run_out = (ctypes.c_int32 * 2)()
+  _native.check(_native.load().msd_op_sampler_step(
+      _ptr(eps), _ptr(z), _ptr(z_split), _ptr(mel_out), _ptr(noise), _ptr(coef), steps, _ptr(step), n,
+      n_dims, passes, float(cond_weight), int(bool(clip_x0)), int(bool(ddim)), float(feat_min),
+      float(feat_max), int(seed) & 0xFFFFFFFFFFFFFFFF, rng_kind, _ptr(rng_keys), n_row, _ptr(row_keys),
+      row_key_stride, _ptr(row_seeds), 0 if run_step is None else first, int(bool(per_row)), launches,
+      run_out, _stream(dev)), 'msd_op_sampler_step')
+  return None if run_step is None else (run_out[0], run_out[1])
+
+
+def op_init_z(z: torch.Tensor, z_split: torch.Tensor, n: int, n_dims: int = 128,
+              init_z: Optional[torch.Tensor] = None, seed: int = 0, rng_kind: int = 0,
+              rng_keys: Optional[torch.Tensor] = None, n_row: int = 0, row_key_stride: int = 0,
+              row_seeds: Optional[torch.Tensor] = None) -> None:
+  """The sampler's initial state (msd_op_init_z): z[:n] = init_z[:n], or the draw of Philox stream 0
+  of seed (rng_kind 0) / of key row 0 of rng_keys (rng_kind 1); n_row > 0: row b's own draw from
+  row_seeds[b] / row_keys + b * row_key_stride (rng_keys is then the per-row table).  z_split[:3 n]
+  gets the [hi | lo | hi] split.  Buffers are checked before the library is called."""
+  _check_state(z, z_split, n, n_dims)
+  dev = z.device
+  if init_z is not None:
+    _check_flat('init_z', init_z, torch.float32, dev, n)
+  else:
+    _check_streams(n, 0, rng_kind, rng_keys, n_row, rng_keys, row_key_stride, row_seeds, n_row > 0, dev)
+  _native.check(_native.load().msd_op_init_z(
+      _ptr(init_z), _ptr(z), _ptr(z_split), n, n_dims, int(seed) & 0xFFFFFFFFFFFFFFFF, rng_kind,
+      _ptr(rng_keys), n_row, row_key_stride, _ptr(row_seeds), _stream(dev)), 'msd_op_init_z')
+
+
+def op_scale_split(feat: torch.Tensor, feat_min: float, feat_max: float,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+  """The encoder's context-feature front end (msd_op_scale_split): feat f32 [rows, n_dims] ->
+  bf16 [rows, 3 n_dims] = [hi | lo | hi] of scale_features(feat, clip=True), written into out (which
+  may be larger: only its first rows * 3 n_dims elements are written) or a new tensor."""
+  if feat.dim() != 2 or not feat.is_cuda:
+    raise ValueError(f'feat: expected a [rows, n_dims] CUDA tensor, got {tuple(feat.shape)} on {feat.device}')
+  rows, nd = feat.shape
+  if rows <= 0 or nd <= 0 or nd % 4:
+    raise ValueError(f'feat: {rows} rows of {nd}: n_dims must be a positive multiple of 4')
+  _check_flat('feat', feat, torch.float32, feat.device, rows * nd)
+  if out is None:
+    out = torch.empty(rows, 3 * nd, dtype=torch.bfloat16, device=feat.device)
+  _check_flat('out', out, torch.bfloat16, feat.device, rows * 3 * nd)
+  _native.check(_native.load().msd_op_scale_split(_ptr(feat), _ptr(out), rows, nd, float(feat_min),
+                                                  float(feat_max), _stream(feat.device)),
+                'msd_op_scale_split')
+  return out
+
+
 def op_jax_bits(seed: int, step: int, n: int, device: torch.device) -> torch.Tensor:
   """Raw uint32 words of the device jax.random stream (as int32 storage; view as uint32)."""
   out = torch.empty(n, dtype=torch.int32, device=device)
