@@ -1637,6 +1637,9 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
       cudaMemsetAsync(tr, 0, 8 * 512 * sizeof(long long), st);
       launch_gemm(ga, st);
       ga.trace = tr;
+      // without the programmatic dependency the traced launch starts after the warm one has
+      // finished, so its main loop does not include waiting for that launch's tail
+      g_pdl_skip_next = true;
       launch_gemm(ga, st);
       ga.trace = nullptr;
       std::vector<long long> h(8 * 512);
@@ -1644,18 +1647,25 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
       cudaMemcpy(h.data(), tr, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
       long long t0 = 0, t1 = 0;
       int n = 0;
-      double sum[5] = {0, 0, 0, 0, 0};
+      double sum[4] = {0, 0, 0, 0};
       for (int b = 0; b < 512; ++b) {
         const long long* r = &h[b * 8];
         if (r[1] == 0) continue;
         if (n == 0 || r[1] < t0) t0 = r[1];
         if (n == 0 || r[2] > t1) t1 = r[2];
-        // r[3] = total cycles; r[4..7] absolute clock64 stamps; entry clock = exit - total
+        // r[3] = total cycles; r[4..7] clock64 offsets from entry
         sum[0] += static_cast<double>(r[3]);
+        sum[1] += static_cast<double>(r[4]);
+        sum[2] += static_cast<double>(r[6] - r[5]);
+        sum[3] += static_cast<double>(r[7] - r[6]);
         ++n;
       }
-      fprintf(stderr, "[gemm trace] M=%d N=%d K=%d epi=%d: %d CTAs, first entry -> last exit %.2f us, mean "
-              "cycles in CTA %.0f\n", M, N, K, epilogue, n, (t1 - t0) * 1e-3, n ? sum[0] / n : 0.0);
+      const double inv_n = n ? 1.0 / n : 0.0;
+      fprintf(stderr, "[gemm trace] M=%d N=%d K=%d epi=%d block_n=%d (automatic %d): %d CTAs, first entry -> "
+              "last exit %.2f us, mean cycles in CTA %.0f: set-up %.0f, main loop %.0f (%.0f per k-block), "
+              "epilogue %.0f\n", M, N, K, epilogue, gemm_resolve_block_n(ga), gemm_pick_wide_bn(M, N), n,
+              (t1 - t0) * 1e-3, sum[0] * inv_n, sum[1] * inv_n, sum[2] * inv_n, sum[2] * inv_n / (K / 64),
+              sum[3] * inv_n);
       for (int b = 0; b < 4 && b < 512; ++b) {
         const long long* r = &h[b * 8];
         if (r[1] == 0) continue;

@@ -29,6 +29,11 @@ constexpr int BLOCK_K = 64;  // 64 bf16 = 128 bytes = one swizzle atom row
 constexpr int MMA_K = 16;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;
 constexpr int GEMM_THREADS = 384;
+// Epilogues that read a row (residual, position table, column gains) issue the loads of
+// EPI_CHUNK column groups together, ahead of the chunk's stores.  Interleaved one by one, every
+// load's latency was paid in full: the compiler cannot move a load above a store to the output,
+// which may alias the row being read (it is the same row for the in-place residual).
+constexpr int EPI_CHUNK = 8;
 
 __host__ __device__ inline bool epi_is_bf16_out(int e) {
   return e == EPI_BF16 || e == EPI_GATED_GELU || e == EPI_GATED_GELU_SPLIT3;
@@ -247,15 +252,26 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                                                  : p.prep.g_hi + st * p.prep.g_hi_step_stride;
       float ssum = 0.f;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = n0 + 8 * j + 2 * q;
-        const float2 x = *reinterpret_cast<const float2*>(out + col);
-        const float2 g = __ldg(reinterpret_cast<const float2*>(gvec + col));
-        const float v0 = acc[4 * j + 2 * h] + x.x, v1 = acc[4 * j + 2 * h + 1] + x.y;
-        ssum = fmaf(v0, v0, ssum);
-        ssum = fmaf(v1, v1, ssum);
-        *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-        *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g.x, v1 * g.y);
+      for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
+        float2 x[EPI_CHUNK], g[EPI_CHUNK];
+#pragma unroll
+        for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+          const int col = n0 + 8 * (j0 + jj) + 2 * q;
+          if (j0 + jj < BN / 8) {
+            x[jj] = *reinterpret_cast<const float2*>(out + col);
+            g[jj] = __ldg(reinterpret_cast<const float2*>(gvec + col));
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+          const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+          if (j >= BN / 8) continue;
+          const float v0 = acc[4 * j + 2 * h] + x[jj].x, v1 = acc[4 * j + 2 * h + 1] + x[jj].y;
+          ssum = fmaf(v0, v0, ssum);
+          ssum = fmaf(v1, v1, ssum);
+          *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+          *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g[jj].x, v1 * g[jj].y);
+        }
       }
       ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
       ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
@@ -276,17 +292,26 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       }
       const bool dup = p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = n0 + 8 * j + 2 * q;
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
+        float2 x[EPI_CHUNK];
         if (add != nullptr) {
-          const float2 x = *reinterpret_cast<const float2*>(add + col);
-          v0 += x.x; v1 += x.y;
+#pragma unroll
+          for (int jj = 0; jj < EPI_CHUNK; ++jj)
+            if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(add + n0 + 8 * (j0 + jj) + 2 * q);
         }
-        *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-        if (dup)
-          *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
-              make_float2(v0, v1);
+#pragma unroll
+        for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+          const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+          if (j >= BN / 8) continue;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (add != nullptr) {
+            v0 += x[jj].x; v1 += x[jj].y;
+          }
+          *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+          if (dup)
+            *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
+                make_float2(v0, v1);
+        }
       }
     }
   }

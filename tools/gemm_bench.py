@@ -7,7 +7,8 @@ lib = _native.load()
 torch.zeros(1, device='cuda')
 EPI = {0: 'bf16', 1: 'f32', 2: 'resid', 3: 'gated'}
 shapes = [('qkv', 4096, 2304, 768, 0), ('wi', 4096, 4096, 768, 3), ('wo', 4096, 768, 2048, 2),
-          ('out', 4096, 768, 768, 2), ('crossq', 2048, 768, 768, 0), ('big', 8192, 8192, 8192, 0),
+          ('out', 4096, 768, 768, 2), ('crossq', 2048, 768, 768, 0), ('crossout', 2048, 768, 768, 2),
+          ('big', 8192, 8192, 8192, 0),
           ('big_k768', 8192, 8192, 768, 0)]
 for name, M, N, K, epi in shapes:
   for variant, bns in ((0, (256, 192, 128, 64)), (1, (256, 128))):
