@@ -409,6 +409,49 @@ int msd_op_audio_resample(const float* x, int32_t rows, int64_t n_in, int32_t or
                           int32_t precision, const double* time_segments, int32_t n_segments,
                           float* y, int64_t n_out, void* stream);
 
+/* Griffin-Lim decoding of MelGAN features: a weight-free stand-in for the vocoder
+ * (audio_codecs.py:249-264, absent), inverting the transform of msd_op_audio_mel.  Four ops on
+ * [rows, F] frames; each refuses (-1) a null pointer, a negative size or iteration count, and more
+ * than 2^31 - 1 frames (rows x F); rows = 0 or F = 0 launches nothing.  All are fp32, asynchronous
+ * on `stream`, and need no context.  A frame's result depends only on its own inputs (and, for
+ * the iteration and ISTFT, its two neighbours'), never on the launch's size or the row's place.
+ *
+ * Magnitude: features [rows, F, 128] f32 device (codec units) -> mag_out [rows, F, 513] f32
+ * device, per frame the non-negative least-squares fit of M = exp(features) by S W (mel_weights
+ * [513, 128] f32 device, linear_to_mel_weight_matrix(128, 513, 16000, 0, 8000)) after n_iter FISTA
+ * steps: Z_0 = Y_0 = max(0, M pinv) (pinv [128, 513] f32 device), Z_{j+1} = max(0, Y_j -
+ * (Y_j W - M) W^T inv_lipschitz), Y_{j+1} = Z_{j+1} + beta[j] (Z_{j+1} - Z_j), mag = Z_{n_iter}.
+ * beta [max(n_iter, 1)] f32 device and inv_lipschitz = 1 / |W|_2^2 come from the host
+ * (audio_codecs.griffin_lim_tables).  A filterbank whose non-zero bands hold more than 2048
+ * weights in all gives NaN. */
+int msd_op_griffin_lim_magnitude(const float* features, int32_t rows, int64_t frames,
+                                 const float* mel_weights, const float* pinv, float inv_lipschitz,
+                                 const float* beta, int32_t n_iter, float* mag_out, void* stream);
+
+/* Phase initialisation (librosa's init='random'): angles [rows, F, 513] complex f32 device
+ * (interleaved re, im) = (cos 2 pi u, sin 2 pi u), u = (r + 0.5) 2^-32 with r word e % 4 of
+ * Philox4x32-10 keyed by seed at counter (e / 4 low, e / 4 high, 0, 0x676c70), e = frame * 513 +
+ * bin within the row: every row draws the same stream. */
+int msd_op_griffin_lim_init(int32_t rows, int64_t frames, uint64_t seed, float* angles, void* stream);
+
+/* n_iter fast Griffin-Lim iterations (librosa.griffinlim's order) on caller-owned state, all
+ * [rows, F, 513] device: mag f32; angles, tprev complex f32, updated in place; work complex f32
+ * scratch.  Each iteration: rebuilt = STFT(ISTFT(mag angles)), a = rebuilt - (momentum / (1 +
+ * momentum)) tprev, tprev = rebuilt, angles = a / (|a| + 1e-16).  STFT is the encoder's: frame k
+ * = samples [320 k, 320 k + 640) of the 320 F-sample signal times window [640] f32 device,
+ * zero-padded to 1024, rfft.  ISTFT is its least-squares inverse (see msd_op_griffin_lim_istft).
+ * Also refused: momentum < 0 (or NaN). */
+int msd_op_griffin_lim_iterate(const float* mag, int32_t rows, int64_t frames, const float* window,
+                               float* angles, float* tprev, float* work, float momentum,
+                               int32_t n_iter, void* stream);
+
+/* audio_out [rows, 320 F] f32 device = ISTFT(mag angles): y[n] = sum_k w[n - 320 k]
+ * irfft(X_k)[n - 320 k] / sum_k w^2[n - 320 k] over the frames k covering n (frame k - 1, then
+ * k), the first 640 samples of each 1024-point irfft; where sum_k w^2 <= 1e-10 (sample 0) the
+ * unnormalised sum. */
+int msd_op_griffin_lim_istft(const float* mag, const float* angles, int32_t rows, int64_t frames,
+                             const float* window, float* audio_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

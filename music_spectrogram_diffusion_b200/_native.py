@@ -19,8 +19,8 @@ _INCLUDE = os.path.join(os.path.dirname(_HERE), 'include')
 LIB_NAME = 'libmsd_b200.so'
 LIB_PATH = os.path.join(_HERE, LIB_NAME)
 SOURCES = ['gemm_wgmma.cu', 'attention_wgmma.cu', 'attention_f32.cu', 'elementwise.cu',
-           'engine.cu', 'audio_mel.cu', 'audio_resample.cu']
-HEADERS = ['common.cuh', 'kernels.h', 'wgmma.cuh']
+           'engine.cu', 'audio_mel.cu', 'audio_resample.cu', 'audio_griffin_lim.cu']
+HEADERS = ['common.cuh', 'kernels.h', 'wgmma.cuh', 'audio_fft.cuh', 'philox.cuh']
 NVCC_FLAGS = [
     '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo',
     '-std=c++17', '-Xcompiler', '-fPIC',
@@ -159,6 +159,12 @@ SYMBOLS = [
     ('msd_op_audio_mel', ctypes.c_int, [_P, _I, ctypes.c_int64, _P, _P, _P, _P]),
     ('msd_op_audio_resample', ctypes.c_int,
      [_P, _I, ctypes.c_int64, _I, _I, _P, _I, _I, _P, _I, _P, ctypes.c_int64, _P]),
+    ('msd_op_griffin_lim_magnitude', ctypes.c_int,
+     [_P, _I, ctypes.c_int64, _P, _P, ctypes.c_float, _P, _I, _P, _P]),
+    ('msd_op_griffin_lim_init', ctypes.c_int, [_I, ctypes.c_int64, ctypes.c_uint64, _P, _P]),
+    ('msd_op_griffin_lim_iterate', ctypes.c_int,
+     [_P, _I, ctypes.c_int64, _P, _P, _P, _P, ctypes.c_float, _I, _P]),
+    ('msd_op_griffin_lim_istft', ctypes.c_int, [_P, _P, _I, ctypes.c_int64, _P, _P, _P]),
 ]
 ABI_VERSION = 6  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
 

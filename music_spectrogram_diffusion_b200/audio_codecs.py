@@ -4,7 +4,11 @@ Mirrors `AudioCodec.scale_features / scale_to_features` (msd/audio_codecs.py:166
 MelGAN constants (204-218).  `MelGAN.encode` is the reference's Audio2Mel (43-143) with MelGAN's
 settings (226-247), computed by the library's CUDA kernel (`engine.op_audio_mel`) from the float32
 tables built here (`hann_window`, `linear_to_mel_weight_matrix`, in TF's order of operations).
-The vocoder (`decode`, a TF-Hub SavedModel, 249-264) is out of scope: it raises.
+The vocoder (`decode`, a TF-Hub SavedModel, 249-264) is out of scope: it raises.  `griffin_lim`
+stands in for it: a weight-free inversion of the encoder's own transform (band-sparse NNLS for the
+linear magnitudes, then fast Griffin-Lim for the phase), computed by the library's CUDA kernels
+(`engine.op_griffin_lim_*`) from the tables built here (`griffin_lim_tables`).  Its audio is not
+the reference's MelGAN audio; it is an audible, deterministic rendering of the features.
 
 Recordings at other rates are brought to 16 kHz by `resample`, librosa 0.9's
 `resample(res_type='kaiser_best')` as the reference calls it (preprocessors.py:150-155, 332-333,
@@ -82,6 +86,107 @@ def mel_tables(device):
             MelGAN.n_dims, MEL_FFT_SIZE // 2 + 1, MelGAN.sample_rate, 0.0,
             float(MelGAN.sample_rate // 2))).to(device))
   return _DEVICE_TABLES[device]
+
+
+# FISTA steps of the mel -> linear-magnitude NNLS: the mean |log(S W) - log M| over bins above 1e-3
+# is below 1e-3 at this count on a synthetic song (tests/test_griffin_lim.py)
+NNLS_ITERS = 200
+
+_GL_HOST: list = []
+_DEVICE_GL_TABLES: Dict[object, Tuple[object, float, object]] = {}
+
+
+def fista_betas(n: int) -> np.ndarray:
+  """FISTA's momentum weights beta_j = (t_j - 1) / t_{j+1}, t_0 = 1,
+  t_{j+1} = (1 + sqrt(1 + 4 t_j^2)) / 2, in fp64: [n]."""
+  t, out = 1.0, np.empty(n, np.float64)
+  for j in range(n):
+    t1 = (1.0 + math.sqrt(1.0 + 4.0 * t * t)) / 2.0
+    out[j] = (t - 1.0) / t1
+    t = t1
+  return out
+
+
+def griffin_lim_host_tables() -> Tuple[np.ndarray, float, np.ndarray]:
+  """(pinv f32 [128, 513], 1 / L as an f32 value, beta f32 [NNLS_ITERS]) of MelGAN's filterbank
+  W (`linear_to_mel_weight_matrix`): pinv(W) and L = |W|_2^2 computed in fp64 from the float32 W,
+  the FISTA weights in fp64; each rounded to float32 once (read-only)."""
+  if not _GL_HOST:
+    w64 = linear_to_mel_weight_matrix(MelGAN.n_dims, MEL_FFT_SIZE // 2 + 1, MelGAN.sample_rate, 0.0,
+                                      float(MelGAN.sample_rate // 2)).astype(np.float64)
+    pinv = np.linalg.pinv(w64).astype(np.float32)
+    inv_l = float(np.float32(1.0 / np.linalg.norm(w64, 2) ** 2))
+    beta = fista_betas(NNLS_ITERS).astype(np.float32)
+    pinv.setflags(write=False)
+    beta.setflags(write=False)
+    _GL_HOST.append((pinv, inv_l, beta))
+  return _GL_HOST[0]
+
+
+def griffin_lim_tables(device):
+  """(pinv f32 [128, 513] tensor, 1 / L float, beta f32 [NNLS_ITERS] tensor) on `device`, built
+  once per device (`griffin_lim_host_tables`)."""
+  if device not in _DEVICE_GL_TABLES:
+    import torch
+    pinv, inv_l, beta = griffin_lim_host_tables()
+    _DEVICE_GL_TABLES[device] = (torch.from_numpy(pinv.copy()).to(device), inv_l,
+                                 torch.from_numpy(beta.copy()).to(device))
+  return _DEVICE_GL_TABLES[device]
+
+
+def griffin_lim(features, n_iter: int = 32, momentum: float = 0.99, seed: int = 0):
+  """MelGAN features [F, 128] or [rows, F, 128] (codec units, as `MelGAN.encode` and
+  `full_pred_encoded` hold them) -> audio f32 [320 F] or [rows, 320 F] at 16 kHz, without the
+  vocoder:
+    1. the linear magnitudes S [F, 513] >= 0, the least-squares fit of exp(features) by S W after
+       NNLS_ITERS FISTA steps from max(0, exp(features) pinv(W));
+    2. random phases from the Philox stream of `seed` (librosa's init='random'; every row draws
+       the same stream, so a row does not depend on its place in the batch);
+    3. n_iter fast Griffin-Lim iterations with `momentum` (librosa.griffinlim's update; 0 is plain
+       Griffin-Lim) through the encoder's own STFT and its least-squares inverse;
+    4. the inverse STFT of S with the final phases.
+  Re-encoding the audio gives F frames again.  The result is deterministic: the same call gives
+  the same bits.  It is not the reference's MelGAN vocoder output.
+
+  Songs of different lengths go in one call padded at the end with `MelGAN.pad_value` to a common
+  F; cut each row to its own num_frames * 320 samples afterwards.  A padded row's last real frame
+  then sees near-silence after it, so it is close to, not bit-identical with, decoding that row
+  alone; equal-length rows are bit-identical.
+
+  A numpy array is decoded on the current CUDA device and comes back as numpy; a CUDA tensor
+  stays on its device.  Raises ValueError for a shape other than [F, 128] or [rows, F, 128],
+  momentum < 0 or n_iter < 0, before any device is used."""
+  import torch
+  from music_spectrogram_diffusion_b200 import engine
+  as_numpy = not torch.is_tensor(features)
+  if as_numpy:
+    features = np.asarray(features)
+  elif not features.is_cuda:
+    raise ValueError('griffin_lim: a tensor must be on a CUDA device (or pass numpy)')
+  if features.ndim not in (2, 3) or features.shape[-1] != MelGAN.n_dims:
+    raise ValueError(f'griffin_lim: features must be [F, {MelGAN.n_dims}] or [rows, F, '
+                     f'{MelGAN.n_dims}], got {tuple(features.shape)}')
+  if not momentum >= 0:
+    raise ValueError(f'griffin_lim: momentum={momentum} must be >= 0')
+  if int(n_iter) != n_iter or n_iter < 0:
+    raise ValueError(f'griffin_lim: n_iter={n_iter} must be an integer >= 0')
+  if as_numpy:
+    dev = torch.device('cuda', torch.cuda.current_device())
+    x = torch.from_numpy(np.ascontiguousarray(features, dtype=np.float32)).to(dev)
+  else:
+    dev = features.device
+    x = features.to(torch.float32).contiguous()
+  rows = x if x.dim() == 3 else x[None]
+  window, weights = mel_tables(dev)
+  pinv, inv_l, beta = griffin_lim_tables(dev)
+  mag = engine.op_griffin_lim_magnitude(rows, weights, pinv, inv_l, beta, NNLS_ITERS)
+  angles = engine.op_griffin_lim_init(rows.shape[0], rows.shape[1], seed, dev)
+  tprev = torch.zeros_like(angles)
+  engine.op_griffin_lim_iterate(mag, window, angles, tprev, momentum, int(n_iter))
+  y = engine.op_griffin_lim_istft(mag, window, angles)
+  if x.dim() == 2:
+    y = y[0]
+  return y.cpu().numpy() if as_numpy else y
 
 
 _KAISER_BEST = []
@@ -237,7 +342,8 @@ class AudioCodec:
     raise NotImplementedError('audio -> mel is outside the DDPM hot path (SURVEY §2)')
 
   def decode(self, features):
-    raise NotImplementedError('mel -> audio vocoder is outside the DDPM hot path (SURVEY §2)')
+    raise NotImplementedError('mel -> audio vocoder is outside the DDPM hot path (SURVEY §2); '
+                              'audio_codecs.griffin_lim renders features to audio without it')
 
   @property
   def context_codec(self):

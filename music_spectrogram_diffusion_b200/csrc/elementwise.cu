@@ -6,6 +6,7 @@
 //   masks            msd/models/diffusion/network.py:28-51, 546; msd/layers.py:341-348
 #include "common.cuh"
 #include "kernels.h"
+#include "philox.cuh"
 
 #define MSD_TRY_RC(expr)      \
   do {                       \
@@ -152,22 +153,8 @@ int launch_norm(const NormDev& p, cudaStream_t stream) {
 }
 
 // ---------------------------------------------------------------------------
-// Philox4x32-10 + Box-Muller (perf-mode noise; parity runs inject noise instead)
+// Philox4x32-10 (philox.cuh) + Box-Muller (perf-mode noise; parity runs inject noise instead)
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3,
-                                              uint32_t k0, uint32_t k1, uint32_t (&out)[4]) {
-  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(M0, c0), lo0 = M0 * c0;
-    const uint32_t hi1 = __umulhi(M1, c2), lo1 = M1 * c2;
-    const uint32_t n0 = hi1 ^ c1 ^ k0, n1 = lo1, n2 = hi0 ^ c3 ^ k1, n3 = lo0;
-    c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-    k0 += W0; k1 += W1;
-  }
-  out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
-
 __device__ __forceinline__ float4 philox_normal4(unsigned long long seed, uint32_t stream,
                                                  unsigned long long idx4) {
   uint32_t r[4];

@@ -1848,6 +1848,65 @@ int msd_op_audio_resample(const float* x, int32_t rows, int64_t n_in, int32_t or
   return 0;
 }
 
+int msd_op_griffin_lim_magnitude(const float* features, int32_t rows, int64_t frames,
+                                 const float* mel_weights, const float* pinv, float inv_lipschitz,
+                                 const float* beta, int32_t n_iter, float* mag_out, void* stream) {
+  MSD_REQUIRE(features && mel_weights && pinv && beta && mag_out,
+              "msd_op_griffin_lim_magnitude: null argument");
+  MSD_REQUIRE(rows >= 0 && frames >= 0 && n_iter >= 0,
+              "msd_op_griffin_lim_magnitude: rows=%d, frames=%lld, n_iter=%d must be >= 0", rows,
+              static_cast<long long>(frames), n_iter);
+  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
+              "msd_op_griffin_lim_magnitude: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
+              static_cast<long long>(frames));
+  MSD_TRY(launch_gl_nnls(features, static_cast<long long>(rows) * frames, mel_weights, pinv,
+                         inv_lipschitz, beta, n_iter, mag_out, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+int msd_op_griffin_lim_init(int32_t rows, int64_t frames, uint64_t seed, float* angles, void* stream) {
+  MSD_REQUIRE(angles, "msd_op_griffin_lim_init: null argument");
+  MSD_REQUIRE(rows >= 0 && frames >= 0, "msd_op_griffin_lim_init: rows=%d, frames=%lld must be >= 0",
+              rows, static_cast<long long>(frames));
+  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
+              "msd_op_griffin_lim_init: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
+              static_cast<long long>(frames));
+  MSD_TRY(launch_gl_phase_init(rows, frames, seed, reinterpret_cast<float2*>(angles),
+                               reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+int msd_op_griffin_lim_iterate(const float* mag, int32_t rows, int64_t frames, const float* window,
+                               float* angles, float* tprev, float* work, float momentum,
+                               int32_t n_iter, void* stream) {
+  MSD_REQUIRE(mag && window && angles && tprev && work, "msd_op_griffin_lim_iterate: null argument");
+  MSD_REQUIRE(rows >= 0 && frames >= 0 && n_iter >= 0,
+              "msd_op_griffin_lim_iterate: rows=%d, frames=%lld, n_iter=%d must be >= 0", rows,
+              static_cast<long long>(frames), n_iter);
+  MSD_REQUIRE(momentum >= 0.f, "msd_op_griffin_lim_iterate: momentum=%g must be >= 0",
+              static_cast<double>(momentum));
+  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
+              "msd_op_griffin_lim_iterate: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
+              static_cast<long long>(frames));
+  MSD_TRY(launch_gl_iterate(mag, rows, frames, window, reinterpret_cast<float2*>(angles),
+                            reinterpret_cast<float2*>(tprev), reinterpret_cast<float2*>(work),
+                            momentum, n_iter, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+int msd_op_griffin_lim_istft(const float* mag, const float* angles, int32_t rows, int64_t frames,
+                             const float* window, float* audio_out, void* stream) {
+  MSD_REQUIRE(mag && angles && window && audio_out, "msd_op_griffin_lim_istft: null argument");
+  MSD_REQUIRE(rows >= 0 && frames >= 0, "msd_op_griffin_lim_istft: rows=%d, frames=%lld must be >= 0",
+              rows, static_cast<long long>(frames));
+  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
+              "msd_op_griffin_lim_istft: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
+              static_cast<long long>(frames));
+  MSD_TRY(launch_gl_istft(mag, reinterpret_cast<const float2*>(angles), rows, frames, window,
+                          audio_out, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
 int msd_op_dense_epilogue(const float* a, const float* w, const float* w1, int32_t M, int32_t N,
                           int32_t K, int32_t epilogue, int32_t block_n, const float* resid,
                           const float* pos, int32_t pos_rows, const int32_t* pos_shift,

@@ -360,5 +360,21 @@ int launch_audio_mel(const float* audio, int rows, long long n_samples, const fl
 int launch_audio_resample(const float* x, int rows, int n_in, double ratio, const double* window,
                           int window_len, int num_table, const double* segments, int n_segments,
                           float* y, int n_out, cudaStream_t stream);
+// Griffin-Lim decoding of MelGAN features (audio_griffin_lim.cu), per frame of `total` = rows x F:
+// features [total, 128] f32 -> magnitude mag [total, 513] f32 by n_iter FISTA steps of NNLS
+// against weights [513, 128] from max(0, exp(features) pinv), pinv [128, 513], beta [n_iter]
+int launch_gl_nnls(const float* features, long long total, const float* weights, const float* pinv,
+                   float inv_l, const float* beta, int n_iter, float* mag, cudaStream_t stream);
+// angles [rows, F, 513] complex f32 = e^{2 pi i u}, u from Philox4x32-10 keyed by seed
+int launch_gl_phase_init(int rows, long long frames, unsigned long long seed, float2* angles,
+                         cudaStream_t stream);
+// n_iter fast Griffin-Lim iterations on angles and tprev [rows, F, 513] complex f32, in place;
+// work is scratch of the same size; window [640] f32
+int launch_gl_iterate(const float* mag, int rows, long long frames, const float* window,
+                      float2* angles, float2* tprev, float2* work, float momentum, int n_iter,
+                      cudaStream_t stream);
+// audio [rows, 320 F] f32 = ISTFT(mag angles)
+int launch_gl_istft(const float* mag, const float2* angles, int rows, long long frames,
+                    const float* window, float* audio, cudaStream_t stream);
 
 }  // namespace msd

@@ -792,3 +792,104 @@ def op_audio_resample(audio: torch.Tensor, orig_sr: int, target_sr: int, window:
         precision, _ptr(segments), segments.shape[0], _ptr(out), out.shape[1],
         _stream(audio.device)), 'msd_op_audio_resample')
   return out
+
+
+def _check_gl(name: str, t: torch.Tensor, dtype, shape, device) -> None:
+  if t.dtype != dtype or not t.is_cuda or not t.is_contiguous():
+    raise ValueError(f'{name}: expected a contiguous {dtype} CUDA tensor, got {t.dtype} on '
+                     f'{t.device} (contiguous: {t.is_contiguous()})')
+  if t.device != device:
+    raise ValueError(f'{name} is on {t.device}, expected {device}')
+  if shape is not None and tuple(t.shape) != tuple(shape):
+    raise ValueError(f'{name}: expected shape {tuple(shape)}, got {tuple(t.shape)}')
+
+
+def op_griffin_lim_magnitude(features: torch.Tensor, weights: torch.Tensor, pinv: torch.Tensor,
+                             inv_lipschitz: float, beta: torch.Tensor, n_iter: int) -> torch.Tensor:
+  """Linear magnitudes of MelGAN features [rows, F, 128] (msd_op_griffin_lim_magnitude): f32
+  [rows, F, 513], the non-negative least-squares fit of exp(features) by S @ weights after n_iter
+  FISTA steps from max(0, exp(features) @ pinv).  weights f32 [513, 128], pinv f32 [128, 513] and
+  beta f32 [>= n_iter] (audio_codecs.griffin_lim_tables) on the features' device.  Enqueued on the
+  device's current stream."""
+  if features.dim() != 3 or features.shape[2] != 128:
+    raise ValueError(f'features: expected [rows, F, 128], got {tuple(features.shape)}')
+  dev = features.device
+  _check_gl('features', features, torch.float32, None, dev)
+  _check_gl('weights', weights, torch.float32, (513, 128), dev)
+  _check_gl('pinv', pinv, torch.float32, (128, 513), dev)
+  _check_gl('beta', beta, torch.float32, None, dev)
+  if int(n_iter) != n_iter or n_iter < 0 or beta.dim() != 1 or beta.shape[0] < max(n_iter, 1):
+    raise ValueError(f'n_iter={n_iter} must be >= 0 with beta [>= max(n_iter, 1)], got beta '
+                     f'{tuple(beta.shape)}')
+  rows, frames = features.shape[:2]
+  out = torch.empty(rows, frames, 513, dtype=torch.float32, device=dev)
+  if out.numel() == 0:
+    return out
+  with torch.cuda.device(dev):
+    _native.check(_native.load().msd_op_griffin_lim_magnitude(
+        _ptr(features), rows, frames, _ptr(weights), _ptr(pinv), float(inv_lipschitz), _ptr(beta),
+        int(n_iter), _ptr(out), _stream(dev)), 'msd_op_griffin_lim_magnitude')
+  return out
+
+
+def op_griffin_lim_init(rows: int, frames: int, seed: int, device: torch.device) -> torch.Tensor:
+  """Random initial phases (msd_op_griffin_lim_init): complex64 [rows, frames, 513] of modulus 1
+  from the Philox stream of seed, the same for every row."""
+  if rows < 0 or frames < 0:
+    raise ValueError(f'rows={rows}, frames={frames} must be >= 0')
+  out = torch.empty(rows, frames, 513, dtype=torch.complex64, device=device)
+  if out.numel() == 0:
+    return out
+  with torch.cuda.device(device):
+    _native.check(_native.load().msd_op_griffin_lim_init(
+        rows, frames, int(seed) & 0xFFFFFFFFFFFFFFFF, _ptr(out), _stream(device)),
+        'msd_op_griffin_lim_init')
+  return out
+
+
+def op_griffin_lim_iterate(mag: torch.Tensor, window: torch.Tensor, angles: torch.Tensor,
+                           tprev: torch.Tensor, momentum: float, n_iter: int,
+                           work: Optional[torch.Tensor] = None) -> None:
+  """n_iter fast Griffin-Lim iterations (msd_op_griffin_lim_iterate) on angles and tprev,
+  complex64 [rows, F, 513], in place, against the magnitudes mag f32 [rows, F, 513] with the
+  codec's window f32 [640].  work (complex64, the same shape) is scratch; one is allocated when it
+  is None.  Enqueued on the device's current stream."""
+  if mag.dim() != 3 or mag.shape[2] != 513:
+    raise ValueError(f'mag: expected [rows, F, 513], got {tuple(mag.shape)}')
+  if not momentum >= 0:
+    raise ValueError(f'momentum={momentum} must be >= 0')
+  if int(n_iter) != n_iter or n_iter < 0:
+    raise ValueError(f'n_iter={n_iter} must be an integer >= 0')
+  dev = mag.device
+  _check_gl('mag', mag, torch.float32, None, dev)
+  _check_gl('window', window, torch.float32, (640,), dev)
+  _check_gl('angles', angles, torch.complex64, mag.shape, dev)
+  _check_gl('tprev', tprev, torch.complex64, mag.shape, dev)
+  if work is None:
+    work = torch.empty_like(angles)
+  _check_gl('work', work, torch.complex64, mag.shape, dev)
+  if mag.numel() == 0 or n_iter == 0:
+    return
+  with torch.cuda.device(dev):
+    _native.check(_native.load().msd_op_griffin_lim_iterate(
+        _ptr(mag), mag.shape[0], mag.shape[1], _ptr(window), _ptr(angles), _ptr(tprev), _ptr(work),
+        float(momentum), int(n_iter), _stream(dev)), 'msd_op_griffin_lim_iterate')
+
+
+def op_griffin_lim_istft(mag: torch.Tensor, window: torch.Tensor, angles: torch.Tensor) -> torch.Tensor:
+  """audio f32 [rows, 320 F] = ISTFT(mag angles) (msd_op_griffin_lim_istft): mag f32 and angles
+  complex64 [rows, F, 513], window f32 [640], on one CUDA device."""
+  if mag.dim() != 3 or mag.shape[2] != 513:
+    raise ValueError(f'mag: expected [rows, F, 513], got {tuple(mag.shape)}')
+  dev = mag.device
+  _check_gl('mag', mag, torch.float32, None, dev)
+  _check_gl('window', window, torch.float32, (640,), dev)
+  _check_gl('angles', angles, torch.complex64, mag.shape, dev)
+  out = torch.empty(mag.shape[0], mag.shape[1] * 320, dtype=torch.float32, device=dev)
+  if out.numel() == 0:
+    return out
+  with torch.cuda.device(dev):
+    _native.check(_native.load().msd_op_griffin_lim_istft(
+        _ptr(mag), _ptr(angles), mag.shape[0], mag.shape[1], _ptr(window), _ptr(out), _stream(dev)),
+        'msd_op_griffin_lim_istft')
+  return out

@@ -4,13 +4,17 @@ Library form of the loops the reference keeps in its colab ("Synthesize Audio" c
 `beam/evaluation.py:156-276`: the first segment runs with a masked context, every later one
 is conditioned on the previous segment's predicted mel; per-segment wall times are reported
 with the reference's `model_timing` fields (first segment excluded, evaluation.py:217-220,
-238-247).  The mel -> audio vocoder is outside this path (SURVEY §2).
+238-247).  The mel -> audio vocoder is outside this path (SURVEY §2); `audio_codecs.griffin_lim`
+stands in for it.
 
 Audio goes the other way through `MelGAN.encode` (the library's CUDA kernel): `load_audio` reads
 a 16 kHz WAV file (or, with resample=True, a WAV file at any rate, resampled to 16 kHz on the GPU
 as the reference's librosa does), `encode_song_audio` gives a recording's ground-truth mels segment by segment
 (`full_gt_encoded`, evaluation.py:156-276), and `context_audio=` primes a song's first segment
 with the end of a recording instead of a masked-out context.
+
+The other way, `audio_codecs.griffin_lim` renders predicted features (`full_pred_encoded`) to
+audio without the absent vocoder, and `save_audio` writes it as a 16-bit WAV file.
 
 `synthesize_songs` runs several such chains at once: each round puts the next segment of every
 active song into one batch, one song per row, and every row draws its noise from its own song's
@@ -84,6 +88,26 @@ def load_audio(path_or_bytes: Union[str, bytes], resample: bool = False) -> np.n
   if rate != 16000:
     x = audio_codecs.resample(x, rate, 16000)
   return x
+
+
+def save_audio(path_or_file, audio, sample_rate: int = 16000) -> None:
+  """Writes mono audio [n] (numpy or a tensor, nominally in [-1, 1)) as a 16-bit PCM WAV file to
+  a path or a writable binary file object: each sample is clipped to [-1, 1), scaled by 32768 and
+  rounded to nearest, so `load_audio` of the file gives the audio quantised to 16 bits back
+  exactly.  NaN is written as 0."""
+  if torch.is_tensor(audio):
+    audio = audio.detach().cpu().numpy()
+  x = np.asarray(audio, np.float64)
+  if x.ndim != 1:
+    raise ValueError(f'save_audio: audio must be mono [n], got shape {x.shape}')
+  if int(sample_rate) != sample_rate or sample_rate <= 0:
+    raise ValueError(f'save_audio: sample_rate={sample_rate} must be a positive integer')
+  q = np.clip(np.rint(np.nan_to_num(x, nan=0.0) * 32768.0), -32768, 32767).astype('<i2')
+  with wave.open(path_or_file, 'wb') as w:
+    w.setnchannels(1)
+    w.setsampwidth(2)
+    w.setframerate(int(sample_rate))
+    w.writeframes(q.tobytes())
 
 
 def encode_song_audio(model, samples: np.ndarray) -> Dict[str, Any]:
