@@ -367,13 +367,9 @@ __device__ __forceinline__ void sampler_step_body(const SamplerArgs& a, int step
   }
 }
 
-__device__ __forceinline__ void prefetch_next_film(const SamplerArgs& a, int step, long long gid) {
+__device__ __forceinline__ void prefetch_next_step(const SamplerArgs& a, int step, long long gid) {
   if (step < 1) return;
   const long long off = gid * 32;  // one 128-byte line per thread and table
-  if (a.film != nullptr && off < a.film_step_floats) {
-    const float* ptr = a.film + static_cast<long long>(step - 1) * a.film_step_floats + off;
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(ptr));
-  }
 #pragma unroll
   for (int t = 0; t < 3; ++t) {
     if (a.pf[t] != nullptr && off < a.pf_step_floats[t]) {
@@ -389,7 +385,7 @@ __global__ void __launch_bounds__(256) sampler_step_kernel(const SamplerArgs a) 
   griddep_wait();
   if (a.run == nullptr) {
     const int step = *a.step;
-    prefetch_next_film(a, step, i4);
+    prefetch_next_step(a, step, i4);
     if (i4 * 4 < a.n) sampler_step_body(a, step, a.noise, a.mel_out, a.seed, i4, false);
     return;
   }
@@ -411,7 +407,7 @@ __global__ void __launch_bounds__(256) sampler_step_kernel(const SamplerArgs a) 
   }
   __syncthreads();
   const int step = s_step;
-  prefetch_next_film(a, step, i4);
+  prefetch_next_step(a, step, i4);
   const float* noise_base = a.run->noise;
   float* mel_base = a.run->mel_out;
   const unsigned long long seed = a.run->seed;

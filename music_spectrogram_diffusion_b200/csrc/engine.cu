@@ -771,37 +771,129 @@ static int run_encoder(msd_ctx* c, const Encoder& e, int B, int len, const uint3
   return 0;
 }
 
-// Cross-attention block of a DecoderLayer (network.py:196-235) over `nseg` conditioned segments:
-// rows x / xn (scratch) / attn (scratch).  concat_encodings attends the concatenated
-// [tokens | context] cache once; sum_cross_attends runs one attention per source (each zeroed
-// where its source is fully masked) and sums them inside the stacked output projection.
-static int cross_attention_block(msd_ctx* c, const DecLayer& w, int l, float* x, bf16* xn, bf16* attn,
-                                 int nseg, cudaStream_t st) {
-  const int d = c->d, hh = c->hh, N = c->N, R = nseg * N;
-  MSD_TRY(norm_into(c, x, w.ln_cross, R, xn, nullptr, 0, st));
-  const size_t kv_off = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;  // elements
+// Cross-attention of the queries in c->qc (the first `nseg` segments) over layer l's K/V cache
+// (network.py:196-235), into `o`, the input buffer of the output projection.  concat_encodings
+// attends the concatenated [tokens | context] cache once; sum_cross_attends runs one attention
+// per source (each zeroed where its source is fully masked) into the two halves of `o`, which the
+// stacked output projection sums.
+static int cross_attention(const msd_ctx* c, int l, int nseg, bf16* o, cudaStream_t st) {
+  const int hh = c->hh, N = c->N, words = c->Mkv / 32;
+  const size_t kv = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;  // elements
   AttnExtra ex;
   ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml;
   ex.kv_static = 1;
-  if (c->cfg.cross_attend_style == 0) {
-    MSD_TRY(dense(c, xn, w.cross_q, R, hh, d, epi_qkv(c), c->qc, hh, nullptr, st));
-    MSD_TRY(attention(c, c->qc, 0, hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh, 2 * hh,
-                      attn, hh, 0, nseg, c->H, N, c->Mkv, c->mask_bits, c->Mkv / 32, st, ex));
-    MSD_TRY(dense(c, attn, w.cross_out, R, d, hh, EPI_RESID_F32, x, d, x, st));
-    return 0;
-  }
-  MSD_TRY(dense(c, xn, w.cross_q, R, 2 * hh, d, epi_qkv(c), c->qc, 2 * hh, nullptr, st));
+  if (c->cfg.cross_attend_style == 0)
+    return attention(c, c->qc, 0, hh, c->kv_cache, kv, 2 * hh, c->kv_cache, kv + hh, 2 * hh, o, hh, 0, nseg,
+                     c->H, N, c->Mkv, c->mask_bits, words, st, ex);
   ex.kv_batch_rows = c->Mkv;
   ex.kv_row0 = 0;
-  MSD_TRY(attention(c, c->qc, 0, 2 * hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh, 2 * hh,
-                    c->attn2, 2 * hh, 0, nseg, c->H, N, c->T, c->mask_bits, c->Mkv / 32, st, ex));
+  MSD_TRY(attention(c, c->qc, 0, 2 * hh, c->kv_cache, kv, 2 * hh, c->kv_cache, kv + hh, 2 * hh, o, 2 * hh, 0,
+                    nseg, c->H, N, c->T, c->mask_bits, words, st, ex));
   ex.kv_row0 = c->T;
   ex.part_o = c->attn_part_o2; ex.part_ml = c->attn_part_ml2;
-  MSD_TRY(attention(c, c->qc, hh, 2 * hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh, 2 * hh,
-                    c->attn2, 2 * hh, hh, nseg, c->H, N, c->C, c->mask_bits + c->T / 32, c->Mkv / 32,
-                    st, ex));
-  MSD_TRY(dense(c, c->attn2, w.cross_out, R, d, 2 * hh, EPI_RESID_F32, x, d, x, st));
-  return 0;
+  return attention(c, c->qc, hh, 2 * hh, c->kv_cache, kv, 2 * hh, c->kv_cache, kv + hh, 2 * hh, o, 2 * hh, hh,
+                   nseg, c->H, N, c->C, c->mask_bits + c->T / 32, words, st, ex);
+}
+
+// A pre-norm (+FiLM) of a decoder layer (layers.py:632-666) takes one of two forms, and only
+// normed_proj and resid_proj below know which.  Stand-alone: an rmsnorm (+FiLM) kernel writes the
+// normalised operand of the projection.  DEFERRED NORMALISATION (bf16 mode, one chain; kernels.h
+// GemmPrep / GemmRowScale): the norm is split into a column gain applied where the residual stream
+// is produced and a row scale + bias row applied where the next projection's accumulator is
+// drained,
+//     (rmsnorm(x) gamma (1 + fs) + fb) W  ==  rsqrt(mean(x^2) + eps) * ((x gamma (1 + fs)) W) + fb W,
+// so no stand-alone rmsnorm kernel runs inside the layers (35 fewer kernels per step).  xn then
+// holds x * g' (unnormalised), and the partial row sums of squares of x are kept in ss_x (the
+// stream entering a layer), ss_so (after the self-attention projection) and ss_co (after the
+// cross-attention one).
+
+// Partial row sums of squares (deferred form): the buffer a residual projection wrote them to and
+// the number of column tiles it summed over
+struct RowSums { float* ss; int parts; };
+
+// One pre-norm site, with what either form needs of it
+struct PreNorm {
+  const float* gamma;  // rmsnorm scale [d]
+  int film;            // its row of the FiLM tables (2l: self-attention, 2l + 1: MLP), or -1: none
+  const float* btab;   // deferred: FiLM bias rows through the projection [steps, Ld, width], or null
+  int width, l;
+  RowSums* lo;         // deferred: the row sums it reads for rows < Rc (the residual projection
+  RowSums* hi;         //   that prepares it writes them there), and those it reads for the others
+};
+
+// Rows [seg0 * N, (seg0 + nseg) * N) of the decoder's buffers, of which the first Rc cross-attend
+struct LayerRows {
+  msd_ctx* c;
+  int Rc;
+  float* x;
+  bf16* xn;
+  cudaStream_t st;
+};
+
+// Deferred form: the column gain gamma (1 + FiLM scale) of a site, with its step stride
+static const float* col_gain(const msd_ctx* c, const PreNorm& p, long long* step_stride) {
+  *step_stride = p.film >= 0 ? static_cast<long long>(2) * c->cfg.num_decoder_layers * c->d : 0;
+  return p.film >= 0 ? c->gtab + static_cast<size_t>(p.film) * c->d : p.gamma;
+}
+
+static GemmArgs deferred_args(const msd_ctx* c, const bf16* A, int lda, const bf16* W, int M, int N, int K,
+                              int epi, void* out, int ldo) {
+  GemmArgs a;
+  memset(&a, 0, sizeof(a));
+  a.A = A; a.B = W; a.M = M; a.N = N; a.K = K; a.lda = lda; a.ldb = K;
+  a.epilogue = epi; a.out = out; a.ldo = ldo; a.step = c->d_step;
+  return a;
+}
+
+// out = (pre-norm p of x) W over the first M rows, W [N, d]
+static int normed_proj(const LayerRows& s, const PreNorm& p, const bf16* W, int M, int N, int epi, void* out,
+                       int ldo) {
+  msd_ctx* c = s.c;
+  const int d = c->d;
+  if (!c->fused_norm) {
+    MSD_TRY(norm_into(c, s.x, p.gamma, M, s.xn, p.film >= 0 ? c->film : nullptr,
+                      p.film >= 0 ? static_cast<long long>(p.film) * 2 * d : 0, s.st));
+    return dense(c, s.xn, W, M, N, d, epi, out, ldo, nullptr, s.st);
+  }
+  if (p.lo->parts == 0) {
+    // no residual epilogue has prepared these rows: layer 0's stream comes from the input projection
+    long long gs = 0;
+    const float* g = col_gain(c, p, &gs);
+    MSD_TRY(launch_prep_rows(s.x, g, gs, c->d_step, M, d, s.xn, d, p.lo->ss, s.st));
+    p.lo->parts = 1;
+  }
+  const int Ld = c->cfg.num_decoder_layers;
+  GemmArgs a = deferred_args(c, s.xn, d, W, M, N, d, epi, out, ldo);
+  a.rs.ss_lo = p.lo->ss; a.rs.parts_lo = p.lo->parts;
+  a.rs.ss_hi = p.hi->ss; a.rs.parts_hi = p.hi->parts;
+  a.rs.split_row = p.lo == p.hi ? M : s.Rc;   // one buffer serves all M rows
+  a.rs.ss_stride = c->passes * c->Bmax * c->N;
+  a.rs.inv_d = 1.0f / static_cast<float>(d);
+  a.rs.col_bias = p.btab ? p.btab + static_cast<size_t>(p.l) * p.width : nullptr;
+  a.rs.bias_step_stride = p.btab ? static_cast<long long>(Ld) * p.width : 0;
+  return launch_gemm(a, s.st);
+}
+
+// x += A W over the first M rows, W [d, K].  Deferred form: the epilogue also prepares the
+// pre-norm that reads x next, lo for rows < split and hi for the others, and writes the row sums
+// where lo reads them (a hi that differs from lo reads its rows from the same buffer).  lo null:
+// no pre-norm follows inside the layers (the decoder_norm reads x itself).
+static int resid_proj(const LayerRows& s, const bf16* A, const bf16* W, int M, int K, const PreNorm* lo,
+                      const PreNorm* hi, int split) {
+  msd_ctx* c = s.c;
+  const int d = c->d;
+  if (!c->fused_norm || lo == nullptr) return dense(c, A, W, M, d, K, EPI_RESID_F32, s.x, d, s.x, s.st);
+  GemmArgs a = deferred_args(c, A, K, W, M, d, K, EPI_RESID_PREP, s.x, d);
+  a.resid = s.x;
+  a.prep.g_lo = col_gain(c, *lo, &a.prep.g_lo_step_stride);
+  a.prep.g_hi = col_gain(c, *hi, &a.prep.g_hi_step_stride);
+  a.prep.split_row = split;
+  a.prep.a = s.xn; a.prep.lda = d;
+  a.prep.ss = lo->lo->ss; a.prep.ss_stride = c->passes * c->Bmax * c->N;
+  const int bn = gemm_resolve_block_n(a);   // the partial row sums are per column tile that runs
+  MSD_REQUIRE(bn > 0, "resid_proj: no tile width for M=%d d=%d", M, d);
+  lo->lo->parts = d / bn;
+  return launch_gemm(a, s.st);
 }
 
 // The 12 DecoderLayers (network.py:161-258) over segments [seg0, seg0 + nseg) of the row buffers.
@@ -810,144 +902,45 @@ static int cross_attention_block(msd_ctx* c, const DecLayer& w, int l, float* x,
 // 0); every other kernel batches all rows.
 static int decoder_layers(msd_ctx* c, int seg0, int nseg, int ncross, cudaStream_t st) {
   const int d = c->d, hh = c->hh, F = c->F, N = c->N, ks = c->ks;
-  const int R = nseg * N;
-  const size_t r0 = static_cast<size_t>(seg0) * N;
-  const int Ld = c->cfg.num_decoder_layers;
-  float* x = c->x + r0 * d;
-  bf16* xn = c->xn + r0 * d * ks;  // [rows, ks*d] view of the scratch buffer (disjoint per range)
-  const size_t qkv_off = r0 * 3 * hh;
-  bf16* attn = c->attn + r0 * hh * ks;
-  bf16* hmid = c->hmid + r0 * F * ks;
-  for (int l = 0; l < Ld; ++l) {
-    const DecLayer& w = c->dec[l];
-    // self-attention block (174-193)
-    MSD_TRY(norm_into(c, x, w.ln_self, R, xn, c->film, static_cast<long long>(2 * l) * 2 * d, st));
-    MSD_TRY(dense(c, xn, w.self_attn.qkv, R, 3 * hh, d, epi_qkv(c), at(c, c->qkv, qkv_off), 3 * hh,
-                  nullptr, st));
-    MSD_TRY(attention(c, c->qkv, qkv_off, 3 * hh, c->qkv, qkv_off + hh, 3 * hh, c->qkv,
-                      qkv_off + 2 * hh, 3 * hh, attn, hh, 0, nseg, c->H, N, N, nullptr, 0, st));
-    MSD_TRY(dense(c, attn, w.self_attn.out, R, d, hh, EPI_RESID_F32, x, d, x, st));
-    // cross-attention block (196-235), conditioned rows only (the first ncross segments)
-    if (ncross > 0) MSD_TRY(cross_attention_block(c, w, l, x, xn, attn, ncross, st));
-    // MLP block (241-256)
-    MSD_TRY(norm_into(c, x, w.ln_mlp, R, xn, c->film, static_cast<long long>(2 * l + 1) * 2 * d, st));
-    MSD_TRY(dense(c, xn, w.mlp.wi, R, 2 * F, d, epi_gated(c), hmid, F * ks, nullptr, st));
-    MSD_TRY(dense(c, hmid, w.mlp.wo, R, d, F, EPI_RESID_F32, x, d, x, st));
-  }
-  return 0;
-}
-
-// The same 12 DecoderLayers with DEFERRED NORMALISATION (bf16 mode, one chain; kernels.h GemmPrep /
-// GemmRowScale): every pre-norm (+FiLM) of layers.py:632-666 is split into a column gain applied
-// where the residual stream is produced and a row scale + bias row applied where the next
-// projection's accumulator is drained,
-//     (rmsnorm(x) gamma (1 + fs) + fb) W  ==  rsqrt(mean(x^2) + eps) * ((x gamma (1 + fs)) W) + fb W,
-// so no stand-alone rmsnorm kernel runs inside the layers (35 fewer kernels per step).
-//   xn      bf16 operand of the next projection: x * g' (unnormalised)
-//   ss_x    row sums of squares of x entering a layer (prep kernel, then each wo projection)
-//   ss_so   ... after the self-attention output projection; ss_co after the cross-attention one
-// Rows of the unconditional pass (>= ncross * N) skip the cross-attention block: their operand for
-// the MLP is written by the self-attention projection already (g_hi), their row sums stay in ss_so.
-static int decoder_layers_fused(msd_ctx* c, int nseg, int ncross, cudaStream_t st) {
-  const int d = c->d, hh = c->hh, F = c->F, N = c->N;
   const int R = nseg * N, Rc = ncross * N;
   const int Ld = c->cfg.num_decoder_layers;
   const int nsrc = c->cfg.cross_attend_style == 1 ? 2 : 1;
-  const long long gstride = static_cast<long long>(2) * Ld * d;
-  const int ss_stride = c->passes * c->Bmax * N;
-  float* x = c->x;
-  bf16* xn = c->xn;
-  auto base_args = [&](const bf16* A, int lda, const bf16* W, int M, int Nn, int K, int epi, void* out,
-                       int ldo) {
-    GemmArgs a;
-    memset(&a, 0, sizeof(a));
-    a.A = A; a.B = W; a.M = M; a.N = Nn; a.K = K; a.lda = lda; a.ldb = K;
-    a.epilogue = epi; a.out = out; a.ldo = ldo; a.step = c->d_step;
-    return a;
+  const size_t r0 = static_cast<size_t>(seg0) * N;
+  // views of the row buffers (disjoint per range); a GEMM-input row is ks x wider
+  const LayerRows s = {c, Rc, c->x + r0 * d, c->xn + r0 * d * ks, st};
+  const size_t qkv_off = r0 * 3 * hh;
+  bf16* attn = c->attn + r0 * hh * ks;
+  bf16* hmid = c->hmid + r0 * F * ks;
+  bf16* cross_o = nsrc == 1 ? attn : c->attn2;
+  RowSums sx = {c->ss_x, 0}, so = {c->ss_so, 0}, co = {c->ss_co, 0};
+  auto self_norm = [&](int l) {
+    return PreNorm{c->dec[l].ln_self, 2 * l, c->btab_qkv, 3 * hh, l, &sx, &sx};
   };
-  // residual projection + operand / row sums for what follows
-  auto resid_prep = [&](const bf16* A, const bf16* W, int M, int K, const float* g_lo, long long s_lo,
-                        const float* g_hi, long long s_hi, int split_row, float* ss, int* parts) {
-    GemmArgs a = base_args(A, K, W, M, d, K, EPI_RESID_PREP, x, d);
-    a.resid = x;
-    a.prep.g_lo = g_lo; a.prep.g_lo_step_stride = s_lo;
-    a.prep.g_hi = g_hi; a.prep.g_hi_step_stride = s_hi;
-    a.prep.split_row = split_row;
-    a.prep.a = xn; a.prep.lda = d;
-    a.prep.ss = ss; a.prep.ss_stride = ss_stride;
-    const int bn = gemm_resolve_block_n(a);   // the partial row sums are per column tile that runs
-    MSD_REQUIRE(bn > 0, "resid_prep: no tile width for M=%d d=%d", M, d);
-    *parts = d / bn;
-    return launch_gemm(a, st);
-  };
-  auto row_scale = [&](GemmArgs& a, const float* lo, int parts_lo, const float* hi, int parts_hi,
-                       int split_row, const float* bias, long long bias_stride) {
-    a.rs.ss_lo = lo; a.rs.parts_lo = parts_lo; a.rs.ss_hi = hi; a.rs.parts_hi = parts_hi;
-    a.rs.split_row = split_row; a.rs.ss_stride = ss_stride; a.rs.inv_d = 1.0f / static_cast<float>(d);
-    a.rs.col_bias = bias; a.rs.bias_step_stride = bias_stride;
-  };
-  // layer 0: the stream comes from the input projection, not from a residual epilogue
-  MSD_TRY(launch_prep_rows(x, c->gtab, gstride, c->d_step, R, d, xn, d, c->ss_x, st));
-  int parts_x = 1, parts_so = 1, parts_co = 1;
   for (int l = 0; l < Ld; ++l) {
     const DecLayer& w = c->dec[l];
-    const float* g_mlp = c->gtab + static_cast<size_t>(2 * l + 1) * d;
+    const PreNorm self = self_norm(l);
+    const PreNorm cross = {w.ln_cross, -1, nullptr, 0, l, &so, &so};
+    // rows that skip the cross-attention keep the row sums of the self-attention projection
+    const PreNorm mlp = {w.ln_mlp, 2 * l + 1, c->btab_wi, 2 * F, l, Rc > 0 ? &co : &so, &so};
     // self-attention block (174-193)
-    {
-      GemmArgs a = base_args(xn, d, w.self_attn.qkv, R, 3 * hh, d, EPI_BF16, c->qkv, 3 * hh);
-      row_scale(a, c->ss_x, parts_x, c->ss_x, parts_x, R, c->btab_qkv + static_cast<size_t>(l) * 3 * hh,
-                static_cast<long long>(Ld) * 3 * hh);
-      MSD_TRY(launch_gemm(a, st));
-    }
-    MSD_TRY(attention(c, c->qkv, 0, 3 * hh, c->qkv, hh, 3 * hh, c->qkv, 2 * hh, 3 * hh, c->attn, hh, 0,
-                      nseg, c->H, N, N, nullptr, 0, st));
-    // x += attn W_out; rows that cross-attend get the cross pre-norm's gain, the others the MLP's
-    MSD_TRY(resid_prep(c->attn, w.self_attn.out, R, hh, Rc > 0 ? w.ln_cross : g_mlp, Rc > 0 ? 0 : gstride,
-                       g_mlp, gstride, Rc, c->ss_so, &parts_so));
+    MSD_TRY(normed_proj(s, self, w.self_attn.qkv, R, 3 * hh, epi_qkv(c), at(c, c->qkv, qkv_off), 3 * hh));
+    MSD_TRY(attention(c, c->qkv, qkv_off, 3 * hh, c->qkv, qkv_off + hh, 3 * hh, c->qkv,
+                      qkv_off + 2 * hh, 3 * hh, attn, hh, 0, nseg, c->H, N, N, nullptr, 0, st));
+    // rows that cross-attend are prepared for the cross-attention's pre-norm, the others for the MLP's
+    MSD_TRY(resid_proj(s, attn, w.self_attn.out, R, hh, Rc > 0 ? &cross : &mlp, &mlp, Rc));
     // cross-attention block (196-235), conditioned rows only
     if (Rc > 0) {
-      GemmArgs a = base_args(xn, d, w.cross_q, Rc, nsrc * hh, d, EPI_BF16, c->qc, nsrc * hh);
-      row_scale(a, c->ss_so, parts_so, c->ss_so, parts_so, Rc, nullptr, 0);
-      MSD_TRY(launch_gemm(a, st));
-      const size_t kv_off = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;
-      AttnExtra ex;
-      ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml;
-      ex.kv_static = 1;
-      if (nsrc == 1) {
-        MSD_TRY(attention(c, c->qc, 0, hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh, 2 * hh,
-                          c->attn, hh, 0, ncross, c->H, N, c->Mkv, c->mask_bits, c->Mkv / 32, st, ex));
-        MSD_TRY(resid_prep(c->attn, w.cross_out, Rc, hh, g_mlp, gstride, g_mlp, gstride, Rc, c->ss_co,
-                           &parts_co));
-      } else {
-        ex.kv_batch_rows = c->Mkv;
-        ex.kv_row0 = 0;
-        MSD_TRY(attention(c, c->qc, 0, 2 * hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh,
-                          2 * hh, c->attn2, 2 * hh, 0, ncross, c->H, N, c->T, c->mask_bits, c->Mkv / 32,
-                          st, ex));
-        ex.kv_row0 = c->T;
-        ex.part_o = c->attn_part_o2; ex.part_ml = c->attn_part_ml2;
-        MSD_TRY(attention(c, c->qc, hh, 2 * hh, c->kv_cache, kv_off, 2 * hh, c->kv_cache, kv_off + hh,
-                          2 * hh, c->attn2, 2 * hh, hh, ncross, c->H, N, c->C, c->mask_bits + c->T / 32,
-                          c->Mkv / 32, st, ex));
-        MSD_TRY(resid_prep(c->attn2, w.cross_out, Rc, 2 * hh, g_mlp, gstride, g_mlp, gstride, Rc,
-                           c->ss_co, &parts_co));
-      }
+      MSD_TRY(normed_proj(s, cross, w.cross_q, Rc, nsrc * hh, epi_qkv(c), c->qc, nsrc * hh));
+      MSD_TRY(cross_attention(c, l, ncross, cross_o, st));
+      MSD_TRY(resid_proj(s, cross_o, w.cross_out, Rc, nsrc * hh, &mlp, &mlp, Rc));
     }
     // MLP block (241-256)
-    {
-      GemmArgs a = base_args(xn, d, w.mlp.wi, R, 2 * F, d, EPI_GATED_GELU, c->hmid, F);
-      if (Rc > 0) row_scale(a, c->ss_co, parts_co, c->ss_so, parts_so, Rc,
-                            c->btab_wi + static_cast<size_t>(l) * 2 * F, static_cast<long long>(Ld) * 2 * F);
-      else row_scale(a, c->ss_so, parts_so, c->ss_so, parts_so, R,
-                     c->btab_wi + static_cast<size_t>(l) * 2 * F, static_cast<long long>(Ld) * 2 * F);
-      MSD_TRY(launch_gemm(a, st));
-    }
+    MSD_TRY(normed_proj(s, mlp, w.mlp.wi, R, 2 * F, epi_gated(c), hmid, F * ks));
     if (l + 1 < Ld) {
-      const float* g_next = c->gtab + static_cast<size_t>(2 * (l + 1)) * d;
-      MSD_TRY(resid_prep(c->hmid, w.mlp.wo, R, F, g_next, gstride, g_next, gstride, R, c->ss_x, &parts_x));
+      const PreNorm next = self_norm(l + 1);
+      MSD_TRY(resid_proj(s, hmid, w.mlp.wo, R, F, &next, &next, R));
     } else {
-      // the decoder_norm that follows is a stand-alone (split-precision) kernel reading x itself
-      MSD_TRY(dense(c, c->hmid, w.mlp.wo, R, d, F, EPI_RESID_F32, x, d, x, st));
+      MSD_TRY(resid_proj(s, hmid, w.mlp.wo, R, F, nullptr, nullptr, R));
     }
   }
   return 0;
@@ -981,8 +974,7 @@ static int run_decoder(msd_ctx* c, int B, int ncond, int total, cudaStream_t st,
     g_pdl_skip_next = true;  // the join kernel has two predecessors
   } else {
     // one chain, both passes batched per kernel except the cross-attention block
-    if (c->fused_norm) MSD_TRY(decoder_layers_fused(c, total, ncond, st));
-    else MSD_TRY(decoder_layers(c, 0, total, ncond, st));
+    MSD_TRY(decoder_layers(c, 0, total, ncond, st));
   }
   // decoder_norm + spec_out_dense in split precision (445-456: fp32 "for stability")
   MSD_TRY(launch_rmsnorm(c->x, c->dec_norm, R, d, c->xn, 3 * d, nullptr, nullptr, 0, 0, 1, st));
@@ -1006,15 +998,15 @@ static int sampler_step(msd_ctx* c, int B, const float* noise, unsigned long lon
   a.row_keys = c->row_keys; a.row_key_stride = 2 * (static_cast<long long>(c->cfg.num_steps) + 1);
   a.row_seeds = c->row_seeds;
   a.run = use_run ? c->run : nullptr;
-  a.film = c->film;
-  a.film_step_floats = static_cast<long long>(2) * c->cfg.num_decoder_layers * 2 * c->d;
+  // the per-step tables the decoder layers read: the FiLM rows, or the deferred normalisation's
+  // tables derived from them
+  const long long Ld = c->cfg.num_decoder_layers;
   if (c->fused_norm) {
-    // the layers read the derived tables instead of the FiLM rows
-    const long long Ld = c->cfg.num_decoder_layers;
-    a.film = nullptr;
     a.pf[0] = c->gtab; a.pf_step_floats[0] = 2 * Ld * c->d;
     a.pf[1] = c->btab_qkv; a.pf_step_floats[1] = Ld * 3 * c->hh;
     a.pf[2] = c->btab_wi; a.pf_step_floats[2] = Ld * 2 * c->F;
+  } else {
+    a.pf[0] = c->film; a.pf_step_floats[0] = 2 * Ld * 2 * c->d;
   }
   if (use_run && c->xrole != 0) {
     a.passes = 2;   // both passes exist, one of them on the peer GPU

@@ -243,12 +243,10 @@ struct SamplerArgs {
   // when non-null: noise / mel_out / seed / step are read from here (device memory) instead of the
   // fields above, and the last block to finish decrements run->step (the step advance)
   RunArgs* run;
-  // FiLM table [num_steps][film_step_floats]: the rows of the NEXT step (147 KB for base) are
-  // prefetched into L2 here, so that the 24 norm kernels of the next step do not each wait for
-  // HBM (the table is 147 MB, every row is read once per call)
-  const float* film; long long film_step_floats;
-  // further per-step tables prefetched the same way (deferred normalisation: column gains and the
-  // two bias-row tables), unused entries null
+  // per-step tables [num_steps][pf_step_floats[t]] the decoder layers read (the FiLM table, or the
+  // deferred normalisation's column gains and two bias-row tables), unused entries null: the rows
+  // of the NEXT step are prefetched into L2 here, so that the next step's kernels do not each wait
+  // for HBM (the FiLM table is 147 MB for base, every row is read once per call)
   const float* pf[3]; long long pf_step_floats[3];
   // Classifier-free guidance split over two GPUs (BASELINE config 5, SURVEY 8e-iii): this GPU ran
   // ONE of the two decoder passes (xrole 1: the conditional one, 2: the unconditional one) and

@@ -1,5 +1,5 @@
 """-m gpu: the attention kernels through the operand views the engine launches them with
-(engine.cu: run_encoder, cross_attention_block, decoder_layers[_fused]) at base dimensions, against
+(engine.cu: run_encoder, cross_attention, decoder_layers) at base dimensions, against
 fp64 attention computed from the same views.
 
 Every case fills the output buffer with a sentinel first (everything outside the written slice
@@ -297,7 +297,7 @@ CROSS_CASES = [(1, 0, 0), (8, 0, 0), (8, 0, 5)]   # (nb, splits, tail): 6 automa
 @pytest.mark.parametrize('bkv', [64, 128])
 @pytest.mark.parametrize('nb,splits,tail', CROSS_CASES)
 def test_concat_cross_attention_from_the_cache(cuda_device, monkeypatch, nb, splits, tail, bkv, logits):
-  """cross_attention_block, concat_encodings: K / V of layer 1 of a 2-layer cache (ld 2 hh, V at
+  """cross_attention, concat_encodings: K / V of layer 1 of a 2-layer cache (ld 2 hh, V at
   column hh), kv_static = 1 (K / V and the mask read ahead of the dependency wait).  'peaked': q
   and k at 2 sigma, logits with sigma ~ 32 (no 1/sqrt(d) in this model), so the running max moves
   across key blocks and splits."""

@@ -1,5 +1,5 @@
-"""-m gpu: the GEMM through every launch form the engine uses (engine.cu: decoder_layers_fused,
-decoder_layers, run_decoder, msd_encode), on caller-owned buffers with the engine's strides,
+"""-m gpu: the GEMM through every launch form the engine uses (engine.cu: decoder_layers
+in both norm forms, run_decoder, msd_encode), on caller-owned buffers with the engine's strides,
 offsets, step-indexed tables and deferred-normalisation arguments (msd_op_gemm_view,
 msd_op_prep_rows), and the load-time conditioning tables behind them (msd_get_conditioning_tables).
 
@@ -445,10 +445,10 @@ LAYER_CASES = ([(B, 'guided', nsrc, plan) for B in (1, 3, 8) for nsrc in (1, 2)
 
 @pytest.mark.parametrize('B,form,nsrc,plan', LAYER_CASES)
 def test_fused_decoder_layer_launches(cuda_device, B, form, nsrc, plan):
-  """decoder_layers_fused, one layer plus the next layer's QKV, every launch as the engine makes it
-  (plan: the engine's automatic tile widths, one width forced wherever it is allowed, or 'mixed':
-  self-out at 192 and cross-out at 64 columns, so the MLP's two row-scale tables have 4 and 12
-  partial sums)."""
+  """decoder_layers in the deferred form, one layer plus the next layer's QKV, every launch as the
+  engine makes it (plan: the engine's automatic tile widths, one width forced wherever it is
+  allowed, or 'mixed': self-out at 192 and cross-out at 64 columns, so the MLP's two row-scale
+  tables have 4 and 12 partial sums)."""
   layer = Layer(B, form, nsrc, cuda_device, seed=1000 * B + 10 * nsrc + len(str(plan)))
   for draw, s in enumerate(TEST_STEPS):
     ran = layer.run(plan, s, draw, loose=(plan == 'auto'))
@@ -585,7 +585,7 @@ def test_input_projections(cuda_device, B, guided):
 
 @pytest.mark.parametrize('B,nsrc', [(1, 1), (3, 2), (8, 1), (8, 2)])
 def test_fp32_accurate_decoder_launches(cuda_device, B, nsrc):
-  """decoder_layers / cross_attention_block in the fp32-accurate mode: every dense is a 3 x bf16
+  """decoder_layers / cross_attention in the fp32-accurate mode: every dense is a 3 x bf16
   split product (K tripled); q / k / v and the cross q come out fp32 (EPI_F32), the residual
   projections add in place (EPI_RESID_F32, cross-out over the first B N rows of 2 B N), the gated
   MLP writes [hi | lo | hi] into ldo = 3F (EPI_GATED_GELU_SPLIT3, exact tanh)."""

@@ -224,11 +224,15 @@ def test_griffin_lim_argument_errors_need_no_device():
 # ---- the shared-header refactor leaves the existing kernels' SASS unchanged ---------------------
 
 PARENT = '371413184d8e1c6c8c43d8c87afdf0143a80cee3'   # the last commit before the shared headers
+HEADERS = 'a730110b2aaf35e5f81c1077848a0c8dbc55ee03'  # the commit that introduced them
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = 'music_spectrogram_diffusion_b200/csrc'
+# kernels changed on purpose since the shared headers came in: compared as that commit built them
+CHANGED_SINCE = {'sampler_step_kernel'}
 
 
 def _sass(root, src, out_dir):
+  """{kernel: SASS} of one source file."""
   cubin = os.path.join(out_dir, src.replace('.cu', '.cubin'))
   cmd = [_native._nvcc()] + _native.NVCC_FLAGS + ['-I', os.path.join(root, 'include'), '-cubin',
                                                   os.path.join(root, CSRC, src), '-o', cubin]
@@ -237,26 +241,39 @@ def _sass(root, src, out_dir):
   sass = subprocess.run([cuobjdump, '-sass', cubin], check=True, capture_output=True,
                         text=True).stdout
   # anonymous-namespace names carry a hash of the source's path
-  return re.sub(r'_GLOBAL__N__[0-9a-f]+_', '_GLOBAL__N__', sass)
+  sass = re.sub(r'_GLOBAL__N__[0-9a-f]+_', '_GLOBAL__N__', sass)
+  parts = re.split(r'^\s+Function : (\S+)\s*$', sass, flags=re.M)
+  return dict(zip(parts[1::2], parts[2::2]))
+
+
+def _checkout(commit, dest):
+  (dest / CSRC).mkdir(parents=True)
+  (dest / 'include').mkdir()
+  listing = subprocess.run(['git', '-C', REPO, 'ls-tree', '--name-only', commit, CSRC + '/'],
+                           check=True, capture_output=True, text=True).stdout.split()
+  for path in listing + ['include/msd_b200.h']:
+    blob = subprocess.run(['git', '-C', REPO, 'show', f'{commit}:{path}'], check=True,
+                          capture_output=True).stdout
+    (dest / path).write_bytes(blob)
+  return str(dest)
 
 
 def test_shared_headers_leave_encoder_and_sampler_sass_unchanged(tmp_path):
   if shutil.which('git') is None or shutil.which(_native._nvcc()) is None:
     pytest.skip('needs git and nvcc')
-  if subprocess.run(['git', '-C', REPO, 'cat-file', '-e', PARENT + '^{commit}'],
-                    capture_output=True).returncode != 0:
-    pytest.skip('the parent commit is not in this checkout')
-  old = tmp_path / 'parent'
-  (old / CSRC).mkdir(parents=True)
-  (old / 'include').mkdir()
-  listing = subprocess.run(['git', '-C', REPO, 'ls-tree', '--name-only', PARENT, CSRC + '/'],
-                           check=True, capture_output=True, text=True).stdout.split()
-  for path in listing + ['include/msd_b200.h']:
-    blob = subprocess.run(['git', '-C', REPO, 'show', f'{PARENT}:{path}'], check=True,
-                          capture_output=True).stdout
-    (old / path).write_bytes(blob)
+  for commit in (PARENT, HEADERS):
+    if subprocess.run(['git', '-C', REPO, 'cat-file', '-e', commit + '^{commit}'],
+                      capture_output=True).returncode != 0:
+      pytest.skip('the commits around the shared headers are not in this checkout')
+  old = _checkout(PARENT, tmp_path / 'parent')
+  at_headers = _checkout(HEADERS, tmp_path / 'headers')
   for src in ('audio_mel.cu', 'elementwise.cu'):
-    a = _sass(str(old), src, str(old))
+    a = _sass(old, src, old)
     b = _sass(REPO, src, str(tmp_path))
-    assert ('audio_mel_kernel' if src == 'audio_mel.cu' else 'sampler_step') in a
-    assert a == b, f'{src}: SASS differs from the parent commit'
+    assert any(('audio_mel_kernel' if src == 'audio_mel.cu' else 'sampler_step') in k for k in a)
+    assert a.keys() == b.keys(), f'{src}: kernels differ from the parent commit'
+    changed = [k for k in a if any(n in k for n in CHANGED_SINCE)]
+    if changed:
+      b.update({k: v for k, v in _sass(at_headers, src, at_headers).items() if k in changed})
+    for k in a:
+      assert a[k] == b[k], f'{src}: SASS of {k} differs from the parent commit'
