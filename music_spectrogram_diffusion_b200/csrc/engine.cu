@@ -1608,6 +1608,19 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
   ga.epilogue = epilogue; ga.out = o; ga.ldo = (epilogue == EPI_GATED_GELU) ? N / 2 : N;
   ga.resid = (variant == 1) ? r : o;  // default variant: in place, like the engine
   ga.variant = variant; ga.block_n = block_n;
+  const bool trace = getenv("MSD_GEMM_TRACE") != nullptr;
+  if (trace && (epilogue == EPI_BF16 || epilogue == EPI_GATED_GELU)) {
+    // traced like the decoder's QKV / cross-q / wi launches: a row scale from one partial sum per
+    // row and a bias row (zero-filled tables)
+    float *ss = nullptr, *bias = nullptr;
+    MSD_TRY(tb.get(&ss, static_cast<size_t>(M)));
+    MSD_TRY(tb.get(&bias, static_cast<size_t>(N)));
+    MSD_CUDA_CHECK(cudaMemset(ss, 0, static_cast<size_t>(M) * 4));
+    MSD_CUDA_CHECK(cudaMemset(bias, 0, static_cast<size_t>(N) * 4));
+    ga.rs.ss_lo = ss; ga.rs.ss_hi = ss; ga.rs.parts_lo = 1; ga.rs.parts_hi = 1;
+    ga.rs.split_row = M; ga.rs.ss_stride = M; ga.rs.inv_d = 1.0f / static_cast<float>(K);
+    ga.rs.col_bias = bias;
+  }
   cudaStream_t st = nullptr;
   MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   cudaEvent_t e0, e1;
@@ -1622,8 +1635,8 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
   float ms = 0.f;
   cudaEventElapsedTime(&ms, e0, e1);
   *ms_out = ms / iters;
-  if (getenv("MSD_GEMM_TRACE") && variant != 1 && rc == 0 && e == cudaSuccess) {
-    // one more launch with per-CTA stamps (after a warm one right before it, like in the loop)
+  if (trace && variant != 1 && rc == 0 && e == cudaSuccess) {
+    // one more launch with per-tile stamps (after a warm one right before it, like in the loop)
     long long* tr = nullptr;
     if (tb.get(&tr, 8 * 512) == 0) {
       cudaMemsetAsync(tr, 0, 8 * 512 * sizeof(long long), st);
@@ -1645,7 +1658,7 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
         if (r[1] == 0) continue;
         if (n == 0 || r[1] < t0) t0 = r[1];
         if (n == 0 || r[2] > t1) t1 = r[2];
-        // r[3] = total cycles; r[4..7] clock64 offsets from entry
+        // r[3] = cycles in the tile; r[4..7] clock64 offsets from its start
         sum[0] += static_cast<double>(r[3]);
         sum[1] += static_cast<double>(r[4]);
         sum[2] += static_cast<double>(r[6] - r[5]);
@@ -1653,15 +1666,15 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
         ++n;
       }
       const double inv_n = n ? 1.0 / n : 0.0;
-      fprintf(stderr, "[gemm trace] M=%d N=%d K=%d epi=%d block_n=%d (automatic %d): %d CTAs, first entry -> "
-              "last exit %.2f us, mean cycles in CTA %.0f: set-up %.0f, main loop %.0f (%.0f per k-block), "
-              "epilogue %.0f\n", M, N, K, epilogue, gemm_resolve_block_n(ga), gemm_pick_wide_bn(M, N), n,
+      fprintf(stderr, "[gemm trace] M=%d N=%d K=%d epi=%d block_n=%d (automatic %d): %d tiles, first start -> "
+              "last end %.2f us, mean cycles per tile %.0f: set-up %.0f, main loop %.0f (%.0f per k-block), "
+              "epilogue %.0f\n", M, N, K, epilogue, gemm_resolve_block_n(ga), gemm_pick_wide_bn(M, N, epilogue), n,
               (t1 - t0) * 1e-3, sum[0] * inv_n, sum[1] * inv_n, sum[2] * inv_n, sum[2] * inv_n / (K / 64),
               sum[3] * inv_n);
       for (int b = 0; b < 4 && b < 512; ++b) {
         const long long* r = &h[b * 8];
         if (r[1] == 0) continue;
-        fprintf(stderr, "[gemm trace]   CTA %d sm %lld: entry +%.2f us, exit +%.2f us; cycles: total %lld, "
+        fprintf(stderr, "[gemm trace]   tile %d sm %lld: start +%.2f us, end +%.2f us; cycles: total %lld, "
                 "setup->wait %lld, wait->acc %lld, acc->stored %lld\n", b, r[0], (r[1] - t0) * 1e-3,
                 (r[2] - t0) * 1e-3, r[3], r[5] - r[4], r[6] - r[5], r[7] - r[6]);
       }

@@ -1,16 +1,19 @@
 // bf16 GEMM on the Hopper tensor cores: D[M,N] = A[M,K] * B[N,K]^T.
 //
-// One CTA per 128 x BN output tile, three warpgroups:
+// Persistent CTAs (at most one per SM), each walking 128 x BN output tiles, three warpgroups:
 //   warpgroup 0 (one lane)  TMA producer: cp.async.bulk.tensor 2D tiles (SWIZZLE_128B) into a
-//                           STAGES-deep smem ring, completion on `full` mbarriers; its register
-//                           allowance goes to the consumers (setmaxnreg)
+//                           STAGES-deep smem ring, completion on `full` mbarriers, running ahead
+//                           into the CTA's next tile; its register allowance goes to the consumers
+//                           (setmaxnreg)
 //   warpgroups 1, 2         consumers: 64 rows each, wgmma.mma_async m64 x nBN x k16 straight from
 //                           the ring (fp32 accumulator fragment in registers), one MMA group kept
 //                           in flight while the previous ring slot is handed back (`empty`), then
 //                           the fused epilogue (residual / gated-GELU / position-add / deferred
 //                           normalisation) from the accumulator fragment: a quad of lanes owns 8
 //                           consecutive columns of a row, so every store covers whole 32-byte
-//                           sectors (fp32) or 16-byte half sectors (bf16)
+//                           sectors (fp32) or 16-byte half sectors (bf16).  The tile's bias row /
+//                           column gains are staged in shared memory (cp.async) during the main
+//                           loop, so the drain's only global loads are the residual / position rows
 //
 // Replaces the XLA dot_general lowering of DenseGeneral (msd/layers.py:397-442) for every
 // projection on the hot path (SURVEY §2.2 K2, K4, K5, K6, K8, K9).
@@ -55,9 +58,7 @@ struct GemmDev {
   int pos_rows;
   const int* pos_shift;
   int dup_rows;
-  // debugging (MSD_GEMM_TRACE with msd_bench_gemm): per CTA 8 int64 -- smid, globaltimer at entry /
-  // exit, total clock64 cycles, then clock64 offsets from entry of: set-up done, main loop entered,
-  // accumulator complete and dependency wait returned, last store issued (first 512 CTAs)
+  // debugging (MSD_GEMM_TRACE with msd_bench_gemm): per-tile stamps, see the kernel
   long long* trace;
   GemmPrep prep;       // EPI_RESID_PREP
   GemmRowScale rs;     // row scale + bias on EPI_BF16 / EPI_GATED_GELU
@@ -70,9 +71,25 @@ struct GemmCfg {
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int STAGE_BUDGET = 200 * 1024;
   static constexpr int STAGES = STAGE_BUDGET / STAGE_BYTES > 6 ? 6 : STAGE_BUDGET / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/ + 1024 /*align*/;
+  static constexpr int CONST_BYTES = 2 /*warpgroups*/ * 2 /*rows*/ * BN * 4;
+  static constexpr int SMEM_BYTES = CONST_BYTES + 1024 /*align*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
 };
 
+// 8-byte asynchronous copy global -> shared (no register round trip); completed by cp_async_wait_all
+__device__ __forceinline__ void cp_async_8(void* smem_dst, const void* gmem_src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// barrier over the 128 threads of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_sync(int wg) {
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+}
+
+// Persistent: gridDim.x CTAs (at most one per SM) walk the 128 x BN output tiles in the static
+// order tile = blockIdx.x + i * gridDim.x, column tiles fastest.  The ring's slot / phase counter
+// runs on across tiles, so the producer streams the next tile's k-blocks while the consumers drain
+// the current one.
 template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
@@ -80,8 +97,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
+  // per consumer warpgroup: the tile's column constants, [0] bias row or g_lo, [1] g_hi (BN each);
+  // addressed from the shared array itself, so that the drain reads them with LDS (generic loads
+  // would be ordered behind its global stores)
+  float* s_const = reinterpret_cast<float*>(smem_raw);
   uint8_t* smem = reinterpret_cast<uint8_t*>(
-      (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+      (reinterpret_cast<uintptr_t>(smem_raw + Cfg::CONST_BYTES) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_STAGE_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + STAGES * Cfg::B_STAGE_BYTES);
@@ -89,20 +110,14 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const int n0 = blockIdx.x * BN;
-  const int m0 = blockIdx.y * BLOCK_M;
+  const int n_tiles = p.N / BN;
+  const int tiles = n_tiles * (p.M / BLOCK_M);
   const int num_kb = p.K / BLOCK_K;
-  const int cta = blockIdx.y * gridDim.x + blockIdx.x;
-  long long* trc = (p.trace != nullptr && threadIdx.x == 128 && cta < 512) ? p.trace + cta * 8 : nullptr;
-  long long t_entry = 0;
-  if (trc) {
-    uint32_t smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    t_entry = clock64();
-    trc[0] = smid; trc[1] = t;
-  }
+  // per-tile stamps, 8 int64 per tile (first 512 tiles): smid, globaltimer at tile start / end,
+  // cycles in the tile, then clock64 offsets from its start of: set-up done (first tile of a CTA
+  // only), main loop entered, accumulator complete and dependency wait returned, last store issued
+  const bool tracing = p.trace != nullptr && threadIdx.x == 128;
+  long long t_tile = tracing ? clock64() : 0;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
@@ -115,31 +130,35 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
     fence_barrier_init();
   }
   __syncthreads();
-  if (trc) trc[4] = clock64() - t_entry;
+  if (tracing && blockIdx.x < 512) p.trace[blockIdx.x * 8 + 4] = clock64() - t_tile;
 
   griddep_launch_dependents();
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == 0 && lane == 0) {
-      // The weight (B) tiles do not depend on the previous kernel: the first ring-full of them is
-      // requested BEFORE griddepcontrol.wait so the fetch overlaps the predecessor's tail.
-      const int prefetched = num_kb < STAGES ? num_kb : STAGES;
-      for (int kb = 0; kb < prefetched; ++kb) {
-        mbar_arrive_expect_tx(&full_bar[kb], Cfg::STAGE_BYTES);
-        tma_load_2d(sB + kb * Cfg::B_STAGE_BYTES, &tmap_b, &full_bar[kb], kb * BLOCK_K, n0);
-      }
-      griddep_wait();
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        if (kb < prefetched) {  // slot was armed and its B tile requested above
-          tma_load_2d(sA + s * A_STAGE_BYTES, &tmap_a, &full_bar[s], kb * BLOCK_K, m0);
-          continue;
+      int it = 0;  // k-blocks loaded so far: ring slot it % STAGES, phase (it / STAGES) & 1
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int n0 = (tile % n_tiles) * BN, m0 = (tile / n_tiles) * BLOCK_M;
+        int kb = 0;
+        if (tile == static_cast<int>(blockIdx.x)) {
+          // The weight (B) tiles do not depend on the previous kernel: the first ring-full of them
+          // is requested BEFORE griddepcontrol.wait so the fetch overlaps the predecessor's tail.
+          const int prefetched = num_kb < STAGES ? num_kb : STAGES;
+          for (int k = 0; k < prefetched; ++k) {
+            mbar_arrive_expect_tx(&full_bar[k], Cfg::STAGE_BYTES);
+            tma_load_2d(sB + k * Cfg::B_STAGE_BYTES, &tmap_b, &full_bar[k], k * BLOCK_K, n0);
+          }
+          griddep_wait();
+          for (; kb < prefetched; ++kb, ++it)
+            tma_load_2d(sA + kb * A_STAGE_BYTES, &tmap_a, &full_bar[kb], kb * BLOCK_K, m0);
         }
-        mbar_wait(&empty_bar[s], ph ^ 1u);
-        mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-        tma_load_2d(sA + s * A_STAGE_BYTES, &tmap_a, &full_bar[s], kb * BLOCK_K, m0);
-        tma_load_2d(sB + s * Cfg::B_STAGE_BYTES, &tmap_b, &full_bar[s], kb * BLOCK_K, n0);
+        for (; kb < num_kb; ++kb, ++it) {
+          const int s = it % STAGES;
+          if (it >= STAGES) mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1u);
+          mbar_arrive_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
+          tma_load_2d(sA + s * A_STAGE_BYTES, &tmap_a, &full_bar[s], kb * BLOCK_K, m0);
+          tma_load_2d(sB + s * Cfg::B_STAGE_BYTES, &tmap_b, &full_bar[s], kb * BLOCK_K, n0);
+        }
       }
     }
     return;
@@ -149,178 +168,227 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int wg = (warp >> 2) - 1;  // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
   const int tid = threadIdx.x & 127;
-  float acc[BN / 2];
-  if (trc) trc[5] = clock64() - t_entry;
-  {
-    const uint64_t da0 = make_smem_desc_sw128(smem_u32(sA) + wg * 64 * 128);
-    const uint64_t db0 = make_smem_desc_sw128(smem_u32(sB));
-    for (int kb = 0; kb < num_kb; ++kb) {
-      const int s = kb % STAGES;
-      mbar_wait(&full_bar[s], (kb / STAGES) & 1);
-      const uint64_t da = da0 + static_cast<uint64_t>(s * (A_STAGE_BYTES >> 4));
-      const uint64_t db = db0 + static_cast<uint64_t>(s * (Cfg::B_STAGE_BYTES >> 4));
-      wgmma_fence_regs(acc);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BLOCK_K / MMA_K; ++k)
-        WgmmaSS<BN>::mma(acc, da + k * 2, db + k * 2, (kb | k) != 0 ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<1>();  // the MMAs of the previous k-block have retired: its slot is free
-      if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[(kb - 1) % STAGES]);
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs(acc);
-  }
-  griddep_wait();  // residual reads / output writes come after the predecessor is complete
-  if (trc) trc[6] = clock64() - t_entry;
-
-  // ---------------- epilogue from the accumulator fragment ----------------
   const int q = lane & 3;
-  const int row_first = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = row_first + 8 * h;
-    if (row >= p.M) continue;
-    // deferred normalisation, consumer side: this row's scale (and the bias row below)
-    float inv_r = 1.0f;
-    const float* bias = nullptr;
-    if (p.rs.ss_lo != nullptr) {
-      const bool lo = row < p.rs.split_row;
-      const float* ssp = (lo ? p.rs.ss_lo : p.rs.ss_hi) + row;
-      const int parts = lo ? p.rs.parts_lo : p.rs.parts_hi;
-      float ss = 0.f;
-      for (int t = 0; t < parts; ++t) ss += ssp[static_cast<size_t>(t) * p.rs.ss_stride];
-      inv_r = rsqrtf(ss * p.rs.inv_d + 1e-6f);
-      if (p.rs.col_bias != nullptr)
-        bias = p.rs.col_bias + (p.step != nullptr ? *p.step : 0) * p.rs.bias_step_stride;
+  float acc[BN / 2];
+  float* cst = s_const + wg * 2 * BN;
+  // The column constants (bias row of the row-scale epilogues, column gains of EPI_RESID_PREP) are
+  // fixed for the whole step -- only the sampler, the step's last kernel, advances the step index,
+  // and the step's first kernel is a plain launch -- so, like the weights, they are requested
+  // before the dependency wait.
+  const long long step = p.step != nullptr ? *p.step : 0;
+  const float* const0 = nullptr;
+  const float* const1 = nullptr;
+  if (p.epilogue == EPI_RESID_PREP) {
+    const0 = p.prep.g_lo + step * p.prep.g_lo_step_stride;
+    const1 = p.prep.g_hi + step * p.prep.g_hi_step_stride;
+  } else if (p.rs.ss_lo != nullptr && p.rs.col_bias != nullptr) {
+    const0 = p.rs.col_bias + step * p.rs.bias_step_stride;
+  }
+  int it = 0;  // k-blocks consumed so far (same count as the producer's)
+  for (int tile = blockIdx.x, i = 0; tile < tiles; tile += gridDim.x, ++i) {
+    const int n0 = (tile % n_tiles) * BN, m0 = (tile / n_tiles) * BLOCK_M;
+    long long* trc = tracing && tile < 512 ? p.trace + tile * 8 : nullptr;
+    if (trc) {
+      long long t;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+      trc[1] = t;
+      trc[5] = clock64() - t_tile;
     }
-    if (p.epilogue == EPI_GATED_GELU || p.epilogue == EPI_GATED_GELU_SPLIT3) {
-      bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
-      const int F = p.N / 2;
+    if (const0 != nullptr) {
+      if (i > 0) warpgroup_sync(wg);  // the previous tile's drain has read its constants
+      for (int c = 2 * tid; c < BN; c += 256) {
+        cp_async_8(cst + c, const0 + n0 + c);
+        if (const1 != nullptr) cp_async_8(cst + BN + c, const1 + n0 + c);
+      }
+    }
+    {
+      const uint64_t da0 = make_smem_desc_sw128(smem_u32(sA) + wg * 64 * 128);
+      const uint64_t db0 = make_smem_desc_sw128(smem_u32(sB));
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const int s = it % STAGES;
+        mbar_wait(&full_bar[s], (it / STAGES) & 1);
+        const uint64_t da = da0 + static_cast<uint64_t>(s * (A_STAGE_BYTES >> 4));
+        const uint64_t db = db0 + static_cast<uint64_t>(s * (Cfg::B_STAGE_BYTES >> 4));
+        wgmma_fence_regs(acc);
+        wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < BN; c += 64) {
+        for (int k = 0; k < BLOCK_K / MMA_K; ++k)
+          WgmmaSS<BN>::mma(acc, da + k * 2, db + k * 2, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the MMAs of the previous k-block have retired: its slot is free
+        if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+    }
+    if (i == 0) griddep_wait();  // residual reads / output writes come after the predecessor is complete
+    if (trc) trc[6] = clock64() - t_tile;
+    if (const0 != nullptr) {
+      cp_async_wait_all();
+      warpgroup_sync(wg);  // every thread's share of the constants has landed
+    }
+
+    // ---------------- epilogue from the accumulator fragment ----------------
+    const int row_first = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    // deferred normalisation, consumer side: both rows' scales before the first store, so the
+    // partial-sum loads are in flight together
+    float inv_r[2] = {1.0f, 1.0f};
+    if (p.rs.ss_lo != nullptr) {
+      const float* ssp[2];
+      int parts[2];
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int jr = c / 8 + jj, jg = jr + 4;
-          float r0 = acc[4 * jr + 2 * h], r1 = acc[4 * jr + 2 * h + 1];
-          float g0 = acc[4 * jg + 2 * h], g1 = acc[4 * jg + 2 * h + 1];
-          if (p.rs.ss_lo != nullptr) {
-            r0 *= inv_r; r1 *= inv_r; g0 *= inv_r; g1 *= inv_r;
-            if (bias != nullptr) {
-              const float2 br = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * jr + 2 * q));
-              const float2 bg = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * jg + 2 * q));
-              r0 += br.x; r1 += br.y; g0 += bg.x; g1 += bg.y;
+      for (int h = 0; h < 2; ++h) {
+        const int row = row_first + 8 * h;
+        const bool lo = row < p.rs.split_row;
+        ssp[h] = (lo ? p.rs.ss_lo : p.rs.ss_hi) + row;
+        parts[h] = lo ? p.rs.parts_lo : p.rs.parts_hi;
+      }
+      float ss[2] = {0.f, 0.f};
+      const int pmax = parts[0] > parts[1] ? parts[0] : parts[1];
+#pragma unroll 4
+      for (int t = 0; t < pmax; ++t) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (t < parts[h]) ss[h] += ssp[h][static_cast<size_t>(t) * p.rs.ss_stride];
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) inv_r[h] = rsqrtf(ss[h] * p.rs.inv_d + 1e-6f);
+    }
+    const bool bias = const0 != nullptr;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row_first + 8 * h;
+      if (p.epilogue == EPI_GATED_GELU || p.epilogue == EPI_GATED_GELU_SPLIT3) {
+        bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
+        const int F = p.N / 2;
+#pragma unroll
+        for (int c = 0; c < BN; c += 64) {
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int jr = c / 8 + jj, jg = jr + 4;
+            float r0 = acc[4 * jr + 2 * h], r1 = acc[4 * jr + 2 * h + 1];
+            float g0 = acc[4 * jg + 2 * h], g1 = acc[4 * jg + 2 * h + 1];
+            if (p.rs.ss_lo != nullptr) {
+              r0 *= inv_r[h]; r1 *= inv_r[h]; g0 *= inv_r[h]; g1 *= inv_r[h];
+              if (bias) {
+                const float2 br = *reinterpret_cast<const float2*>(cst + 8 * jr + 2 * q);
+                const float2 bg = *reinterpret_cast<const float2*>(cst + 8 * jg + 2 * q);
+                r0 += br.x; r1 += br.y; g0 += bg.x; g1 += bg.y;
+              }
+            }
+            const int oc = (n0 + c) / 2 + 8 * jj + 2 * q;
+            if (p.epilogue == EPI_GATED_GELU) {
+              *reinterpret_cast<uint32_t*>(out + oc) = pack_bf16(gelu_tanh(r0) * g0, gelu_tanh(r1) * g1);
+            } else {
+              // fp32-accurate mode: exact tanh, result kept to ~16 mantissa bits as [hi | lo | hi]
+              const float v0 = gelu_tanh_exact(r0) * g0, v1 = gelu_tanh_exact(r1) * g1;
+              const uint32_t hi = pack_bf16(v0, v1);
+              const uint32_t lo = pack_bf16(v0 - __bfloat162float(__float2bfloat16_rn(v0)),
+                                            v1 - __bfloat162float(__float2bfloat16_rn(v1)));
+              *reinterpret_cast<uint32_t*>(out + oc) = hi;
+              *reinterpret_cast<uint32_t*>(out + F + oc) = lo;
+              *reinterpret_cast<uint32_t*>(out + 2 * F + oc) = hi;
             }
           }
-          const int oc = (n0 + c) / 2 + 8 * jj + 2 * q;
-          if (p.epilogue == EPI_GATED_GELU) {
-            *reinterpret_cast<uint32_t*>(out + oc) = pack_bf16(gelu_tanh(r0) * g0, gelu_tanh(r1) * g1);
-          } else {
-            // fp32-accurate mode: exact tanh, result kept to ~16 mantissa bits as [hi | lo | hi]
-            const float v0 = gelu_tanh_exact(r0) * g0, v1 = gelu_tanh_exact(r1) * g1;
-            const uint32_t hi = pack_bf16(v0, v1);
-            const uint32_t lo = pack_bf16(v0 - __bfloat162float(__float2bfloat16_rn(v0)),
-                                          v1 - __bfloat162float(__float2bfloat16_rn(v1)));
-            *reinterpret_cast<uint32_t*>(out + oc) = hi;
-            *reinterpret_cast<uint32_t*>(out + F + oc) = lo;
-            *reinterpret_cast<uint32_t*>(out + 2 * F + oc) = hi;
-          }
         }
-      }
-    } else if (p.epilogue == EPI_BF16) {
-      bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
+      } else if (p.epilogue == EPI_BF16) {
+        bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = n0 + 8 * j + 2 * q;
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (p.rs.ss_lo != nullptr) {
-          v0 *= inv_r; v1 *= inv_r;
-          if (bias != nullptr) {
-            const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + col));
-            v0 += b2.x; v1 += b2.y;
-          }
-        }
-        *reinterpret_cast<uint32_t*>(out + col) = pack_bf16(v0, v1);
-      }
-    } else if (p.epilogue == EPI_RESID_PREP) {
-      // deferred normalisation, producer side: x = acc + residual (in place), the next GEMM's
-      // operand bf16(x * g) and this tile's share of the row's sum of squares
-      float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
-      bf16* arow = p.prep.a + static_cast<size_t>(row) * p.prep.lda;
-      const long long st = p.step != nullptr ? *p.step : 0;
-      const float* gvec = row < p.prep.split_row ? p.prep.g_lo + st * p.prep.g_lo_step_stride
-                                                 : p.prep.g_hi + st * p.prep.g_hi_step_stride;
-      float ssum = 0.f;
-#pragma unroll
-      for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
-        float2 x[EPI_CHUNK], g[EPI_CHUNK];
-#pragma unroll
-        for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-          const int col = n0 + 8 * (j0 + jj) + 2 * q;
-          if (j0 + jj < BN / 8) {
-            x[jj] = *reinterpret_cast<const float2*>(out + col);
-            g[jj] = __ldg(reinterpret_cast<const float2*>(gvec + col));
-          }
-        }
-#pragma unroll
-        for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-          const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
-          if (j >= BN / 8) continue;
-          const float v0 = acc[4 * j + 2 * h] + x[jj].x, v1 = acc[4 * j + 2 * h + 1] + x[jj].y;
-          ssum = fmaf(v0, v0, ssum);
-          ssum = fmaf(v1, v1, ssum);
-          *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-          *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g[jj].x, v1 * g[jj].y);
-        }
-      }
-      ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
-      ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
-      if (q == 0) p.prep.ss[static_cast<size_t>(n0 / BN) * p.prep.ss_stride + row] = ssum;
-    } else {
-      float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
-      const float* add = nullptr;  // row added to the accumulator
-      if (p.epilogue == EPI_RESID_F32) {
-        add = p.resid + static_cast<size_t>(row) * p.ldo;
-      } else if (p.epilogue == EPI_POS_F32) {
-        const int seq = row / p.pos_rows;
-        int pr = row - seq * p.pos_rows;
-        if (p.pos_shift != nullptr) {
-          pr -= p.pos_shift[seq];
-          if (pr < 0) pr += p.pos_rows;
-        }
-        add = p.pos + static_cast<size_t>(pr) * p.N;
-      }
-      const bool dup = p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
-#pragma unroll
-      for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
-        float2 x[EPI_CHUNK];
-        if (add != nullptr) {
-#pragma unroll
-          for (int jj = 0; jj < EPI_CHUNK; ++jj)
-            if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(add + n0 + 8 * (j0 + jj) + 2 * q);
-        }
-#pragma unroll
-        for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-          const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
-          if (j >= BN / 8) continue;
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n0 + 8 * j + 2 * q;
           float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-          if (add != nullptr) {
-            v0 += x[jj].x; v1 += x[jj].y;
+          if (p.rs.ss_lo != nullptr) {
+            v0 *= inv_r[h]; v1 *= inv_r[h];
+            if (bias) {
+              const float2 b2 = *reinterpret_cast<const float2*>(cst + 8 * j + 2 * q);
+              v0 += b2.x; v1 += b2.y;
+            }
           }
-          *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-          if (dup)
-            *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
-                make_float2(v0, v1);
+          *reinterpret_cast<uint32_t*>(out + col) = pack_bf16(v0, v1);
+        }
+      } else if (p.epilogue == EPI_RESID_PREP) {
+        // deferred normalisation, producer side: x = acc + residual (in place), the next GEMM's
+        // operand bf16(x * g) and this tile's share of the row's sum of squares
+        float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
+        bf16* arow = p.prep.a + static_cast<size_t>(row) * p.prep.lda;
+        const float* gvec = row < p.prep.split_row ? cst : cst + BN;
+        float ssum = 0.f;
+#pragma unroll
+        for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
+          float2 x[EPI_CHUNK];
+#pragma unroll
+          for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+            const int col = n0 + 8 * (j0 + jj) + 2 * q;
+            if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(out + col);
+          }
+#pragma unroll
+          for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+            const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+            if (j >= BN / 8) continue;
+            const float v0 = acc[4 * j + 2 * h] + x[jj].x, v1 = acc[4 * j + 2 * h + 1] + x[jj].y;
+            const float2 g = *reinterpret_cast<const float2*>(gvec + 8 * j + 2 * q);
+            ssum = fmaf(v0, v0, ssum);
+            ssum = fmaf(v1, v1, ssum);
+            *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+            *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g.x, v1 * g.y);
+          }
+        }
+        ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
+        ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
+        if (q == 0) p.prep.ss[static_cast<size_t>(n0 / BN) * p.prep.ss_stride + row] = ssum;
+      } else {
+        float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
+        const float* add = nullptr;  // row added to the accumulator
+        if (p.epilogue == EPI_RESID_F32) {
+          add = p.resid + static_cast<size_t>(row) * p.ldo;
+        } else if (p.epilogue == EPI_POS_F32) {
+          const int seq = row / p.pos_rows;
+          int pr = row - seq * p.pos_rows;
+          if (p.pos_shift != nullptr) {
+            pr -= p.pos_shift[seq];
+            if (pr < 0) pr += p.pos_rows;
+          }
+          add = p.pos + static_cast<size_t>(pr) * p.N;
+        }
+        const bool dup = p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
+#pragma unroll
+        for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
+          float2 x[EPI_CHUNK];
+          if (add != nullptr) {
+#pragma unroll
+            for (int jj = 0; jj < EPI_CHUNK; ++jj)
+              if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(add + n0 + 8 * (j0 + jj) + 2 * q);
+          }
+#pragma unroll
+          for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+            const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+            if (j >= BN / 8) continue;
+            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if (add != nullptr) {
+              v0 += x[jj].x; v1 += x[jj].y;
+            }
+            *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+            if (dup)
+              *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
+                  make_float2(v0, v1);
+          }
         }
       }
     }
-  }
-  if (trc) {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    trc[2] = t;
-    trc[7] = clock64() - t_entry;
-    trc[3] = trc[7];
+    if (tracing) {
+      const long long t_end = clock64();
+      if (trc) {
+        uint32_t smid;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+        long long t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+        trc[0] = smid;
+        trc[2] = t;
+        trc[3] = trc[7] = t_end - t_tile;
+      }
+      t_tile = t_end;
+    }
   }
 }
 
@@ -342,7 +410,9 @@ template <int BN>
 int launch_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& d, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
   static_assert(Cfg::SMEM_BYTES <= 227 * 1024 && Cfg::STAGES >= 3, "smem budget");
-  dim3 grid(d.N / BN, (d.M + BLOCK_M - 1) / BLOCK_M);
+  const int tiles = (d.N / BN) * (d.M / BLOCK_M);
+  const int sms = gemm_sm_count();
+  dim3 grid(tiles < sms ? tiles : sms);
   ProfScope prof(KC_GEMM, 2.0 * d.M * d.N * d.K,
                  2.0 * (static_cast<double>(d.M) * d.K + static_cast<double>(d.N) * d.K) +
                      4.0 * d.M * d.N, st);
@@ -370,20 +440,23 @@ int gemm_configure() {
   return configure_bn<256>();
 }
 
-// Tile width of the default variant: the widest tile re-reads the least of A and B per FLOP, unless
-// it leaves SMs idle that a narrower tiling would use: among the widths whose tile count fits the
-// SMs (one CTA each), take the one with the most tiles.
-int gemm_pick_wide_bn(int M, int N) {
+// Tile width of the default variant.  The CTAs are persistent, one per SM, so a launch takes
+// ceil(tiles / SMs) tile times, and a tile's k-block costs about 4 (BN + 64) cycles (measured 515 /
+// 690 / 983 / 1168 at BN 64 / 128 / 192 / 256): take the width with the least
+// ceil(tiles / SMs) * (BN + 64), the wider one on a tie (it re-reads the least of A and B per FLOP).
+// 96 only for the fp32-output epilogues.
+int gemm_pick_wide_bn(int M, int N, int epilogue) {
   const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-  const int widths[4] = {256, 192, 128, 64};
-  const int conc = gemm_sm_count();
-  int best = 0, best_tiles = 0;
-  for (int i = 0; i < 4; ++i) {
+  const int widths[5] = {256, 192, 128, 96, 64};
+  const int sms = gemm_sm_count();
+  int best = 0;
+  long long best_cost = 0;
+  for (int i = 0; i < 5; ++i) {
     const int bn = widths[i];
-    if (N % bn != 0) continue;
-    const int tiles = m_tiles * (N / bn);
-    if (best == 0) { best = bn; best_tiles = tiles; continue; }   // widest dividing width
-    if (best_tiles < conc && tiles <= conc && tiles > best_tiles) { best = bn; best_tiles = tiles; }
+    if (N % bn != 0 || (bn == 96 && epi_is_bf16_out(epilogue))) continue;
+    const long long tiles = static_cast<long long>(m_tiles) * (N / bn);
+    const long long cost = (tiles + sms - 1) / sms * (bn + 64);
+    if (best == 0 || cost < best_cost) { best = bn; best_cost = cost; }
   }
   return best;
 }
@@ -410,7 +483,7 @@ static bool gemm_wide_variant(const GemmArgs& a) {
 int gemm_resolve_block_n(const GemmArgs& a) {
   const bool wide = gemm_wide_variant(a);
   const int bn = a.block_n ? a.block_n
-                           : (wide ? gemm_pick_wide_bn(a.M, a.N) : gemm_pick_block_n(a.M, a.N));
+                           : (wide ? gemm_pick_wide_bn(a.M, a.N, a.epilogue) : gemm_pick_block_n(a.M, a.N));
   const bool allowed = bn == 64 || bn == 128 || bn == 256 || (wide && bn == 192) ||
                        (wide && bn == 96 && !epi_is_bf16_out(a.epilogue));
   return allowed && a.N % bn == 0 ? bn : 0;

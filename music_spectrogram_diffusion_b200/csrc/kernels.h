@@ -131,9 +131,9 @@ struct GemmArgs {
   const CUtensorMap* tmap_a;
   const CUtensorMap* tmap_b;
   int block_n;           // 0 = auto
-  int variant;           // tile-width choice: 0 = widest that fills the SMs (default, 96 / 192 allowed),
+  int variant;           // tile-width choice: 0 = fewest waves of tiles (default, 96 / 192 allowed),
                          // 1 = power-of-two widths only
-  long long* trace;      // debugging: per-CTA stamps (8 int64 per CTA, first 512 CTAs), or null
+  long long* trace;      // debugging: per-tile stamps (8 int64 per tile, first 512 tiles), or null
   // deferred normalisation: prep.a != null with EPI_RESID_PREP; rs.ss_lo != null
   // with EPI_BF16 / EPI_GATED_GELU; `step` is the device step index the strides multiply
   GemmPrep prep;
@@ -144,7 +144,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream);
 int gemm_configure();  // opt in to the kernels' dynamic shared memory sizes (idempotent)
 // Box rows the A / B maps must be built with for a given block_n choice.
 int gemm_pick_block_n(int M, int N);
-int gemm_pick_wide_bn(int M, int N);
+int gemm_pick_wide_bn(int M, int N, int epilogue);
 // The tile width launch_gemm(a) runs with (a.block_n, a.variant, MSD_GEMM_VARIANT and the shape),
 // or 0 when that width is not allowed.  Whoever sizes per-tile outputs (EPI_RESID_PREP's partial
 // row sums: N / width of them) must take the width from here.
