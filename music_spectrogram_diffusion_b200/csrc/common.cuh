@@ -116,6 +116,28 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// TMA stores shared -> global, tracked per issuing thread in bulk async-groups.  Generic-proxy
+// writes to the source must be made visible to the async proxy first (fence_proxy_async_smem,
+// then a barrier over the writers); wait_group_read<N> returns once at most N of the thread's
+// groups still read shared memory, wait_group_all once all of them have completed their writes.
+__device__ __forceinline__ void fence_proxy_async_smem() {
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() {
+  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// all of the thread's groups complete (at a kernel's exit: no memory clobber, nothing follows)
+__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;"); }
+
 // ----------------------------------------------------------------------------
 // wgmma shared-memory matrix descriptors (PTX ISA "asynchronous warpgroup-level matrix
 // shared memory layout / matrix descriptor")

@@ -77,8 +77,8 @@ static int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint6
                         uint64_t ld, uint32_t box_rows, int elem_bytes, int inner_bytes = 128);
 
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                      uint64_t ld, uint32_t box_rows) {
-  return make_tmap_2d(out, base, rows, cols, ld, box_rows, 2);
+                      uint64_t ld, uint32_t box_rows, int inner_bytes) {
+  return make_tmap_2d(out, base, rows, cols, ld, box_rows, 2, inner_bytes);
 }
 
 static int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
@@ -1677,6 +1677,17 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
         fprintf(stderr, "[gemm trace]   tile %d sm %lld: start +%.2f us, end +%.2f us; cycles: total %lld, "
                 "setup->wait %lld, wait->acc %lld, acc->stored %lld\n", b, r[0], (r[1] - t0) * 1e-3,
                 (r[2] - t0) * 1e-3, r[3], r[5] - r[4], r[6] - r[5], r[7] - r[6]);
+      }
+      // the tiles of CTA 0 in order: main loop, drain (bf16 outputs: until the last sub-tile is
+      // handed to TMA, whose global writes then run under the next tile's main loop)
+      int sms = 0;
+      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+      const int grid = std::min(n, sms > 0 ? sms : n);
+      for (int b = 0, i = 0; grid > 0 && b < 512; b += grid, ++i) {
+        const long long* r = &h[b * 8];
+        if (r[1] == 0) break;
+        fprintf(stderr, "[gemm trace]   CTA 0 tile %d (#%d): start +%.2f us; cycles: main loop %lld, drain %lld\n",
+                i, b, (r[1] - t0) * 1e-3, r[6] - r[5], r[7] - r[6]);
       }
     }
   }

@@ -9,9 +9,10 @@
 //                           the ring (fp32 accumulator fragment in registers), one MMA group kept
 //                           in flight while the previous ring slot is handed back (`empty`), then
 //                           the fused epilogue (residual / gated-GELU / position-add / deferred
-//                           normalisation) from the accumulator fragment: a quad of lanes owns 8
-//                           consecutive columns of a row, so every store covers whole 32-byte
-//                           sectors (fp32) or 16-byte half sectors (bf16).  The tile's bias row /
+//                           normalisation) from the accumulator fragment: bf16 outputs through
+//                           shared-memory staging and TMA stores the drain does not wait for; fp32
+//                           outputs straight from the fragment, a quad of lanes owning 8
+//                           consecutive columns of a row (whole 32-byte sectors).  The tile's bias row /
 //                           column gains are staged in shared memory (cp.async) during the main
 //                           loop, so the drain's only global loads are the residual / position rows
 //
@@ -37,6 +38,9 @@ constexpr int GEMM_THREADS = 384;
 // load's latency was paid in full: the compiler cannot move a load above a store to the output,
 // which may alias the row being read (it is the same row for the in-place residual).
 constexpr int EPI_CHUNK = 8;
+// The bf16 outputs leave through shared memory: each consumer warpgroup owns two staging buffers
+// of one 64-row x 32-column sub-tile (64-byte rows, the box of the SWIZZLE_64B output map).
+constexpr int STG_BUF_BYTES = 64 * 64;
 
 __host__ __device__ inline bool epi_is_bf16_out(int e) {
   return e == EPI_BF16 || e == EPI_GATED_GELU || e == EPI_GATED_GELU_SPLIT3;
@@ -72,13 +76,20 @@ struct GemmCfg {
   static constexpr int STAGE_BUDGET = 200 * 1024;
   static constexpr int STAGES = STAGE_BUDGET / STAGE_BYTES > 6 ? 6 : STAGE_BUDGET / STAGE_BYTES;
   static constexpr int CONST_BYTES = 2 /*warpgroups*/ * 2 /*rows*/ * BN * 4;
-  static constexpr int SMEM_BYTES = CONST_BYTES + 1024 /*align*/ + STAGES * STAGE_BYTES + 256 /*barriers*/;
+  // the staging buffers fit between the ring budget and the 227 KB limit at every width, so they
+  // cost no ring stage (6 / 6 / 6 / 5 / 4 stages at BN 64 / 96 / 128 / 192 / 256)
+  static constexpr int STG_BYTES = 2 /*warpgroups*/ * 2 * STG_BUF_BYTES;
+  static constexpr int SMEM_BYTES =
+      CONST_BYTES + 1024 /*align*/ + STAGES * STAGE_BYTES + STG_BYTES + 256 /*barriers*/;
 };
 
 // 8-byte asynchronous copy global -> shared (no register round trip); completed by cp_async_wait_all
 __device__ __forceinline__ void cp_async_8(void* smem_dst, const void* gmem_src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src)
                : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 // barrier over the 128 threads of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
@@ -93,7 +104,8 @@ __device__ __forceinline__ void warpgroup_sync(int wg) {
 template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                       const __grid_constant__ CUtensorMap tmap_b, const GemmDev p) {
+                       const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_o, const GemmDev p) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -105,7 +117,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       (reinterpret_cast<uintptr_t>(smem_raw + Cfg::CONST_BYTES) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + STAGES * Cfg::B_STAGE_BYTES);
+  uint8_t* s_stg = sB + STAGES * Cfg::B_STAGE_BYTES;  // 1024-aligned, as the swizzle pattern needs
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_stg + Cfg::STG_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
@@ -115,13 +128,15 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const int num_kb = p.K / BLOCK_K;
   // per-tile stamps, 8 int64 per tile (first 512 tiles): smid, globaltimer at tile start / end,
   // cycles in the tile, then clock64 offsets from its start of: set-up done (first tile of a CTA
-  // only), main loop entered, accumulator complete and dependency wait returned, last store issued
+  // only), main loop entered, accumulator complete and dependency wait returned, last sub-tile
+  // handed to TMA (bf16 outputs) / last store issued (fp32 outputs)
   const bool tracing = p.trace != nullptr && threadIdx.x == 128;
   long long t_tile = tracing ? clock64() : 0;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if (epi_is_bf16_out(p.epilogue)) tma_prefetch_desc(&tmap_o);
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
@@ -256,14 +271,38 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
       for (int h = 0; h < 2; ++h) inv_r[h] = rsqrtf(ss[h] * p.rs.inv_d + 1e-6f);
     }
     const bool bias = const0 != nullptr;
+    // bf16 outputs: one 64 x 32 sub-tile at a time into the staging buffer, then lane 0 of the
+    // warpgroup hands it to the TMA unit and the drain moves on without waiting for the global
+    // writes; after the last sub-tile the warpgroup goes straight into the next tile's main loop.
+    // Before the barrier that releases sub-tile k, lane 0 waits until the store of sub-tile k - 1
+    // has read the other buffer, which sub-tile k + 1 overwrites.  Sub-tile s of a tile uses buffer
+    // s & 1; after an odd count the next tile's first sub-tile waits for the last store's read.
+    // this warpgroup's two staging buffers, and the thread's place in them: the 16-byte chunk c of
+    // local row r sits at chunk c ^ ((r >> 1) & 3) (SWIZZLE_64B), so the 4-byte writes of a warp
+    // (8 rows x 4 lanes, one chunk per row) fall on 32 distinct banks.  Bits 4-5 of the thread's
+    // address hold its row's (r >> 1) & 3, so XOR-ing the chunk into them places it.
+    uint8_t* const stg = s_stg + wg * 2 * STG_BUF_BYTES;
+    const int stg_row = (warp & 3) * 16 + (lane >> 2);
+    const uint32_t stg_thr = smem_u32(stg) + stg_row * 64 + (((stg_row >> 1) & 3) << 4) + 4 * q;
+    const int stg_m = m0 + wg * 64;
+    auto stg_put = [&](int b, int h, int jj, uint32_t v) {
+      st_shared_u32((stg_thr ^ (jj << 4)) + b * STG_BUF_BYTES + h * 8 * 64, v);
+    };
+    auto stg_release = [&]() {
+      fence_proxy_async_smem();
+      if (tid == 0) bulk_wait_group_read<0>();
+      warpgroup_sync(wg);
+    };
+    if (p.epilogue == EPI_GATED_GELU) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = row_first + 8 * h;
-      if (p.epilogue == EPI_GATED_GELU || p.epilogue == EPI_GATED_GELU_SPLIT3) {
-        bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
-        const int F = p.N / 2;
+      for (int c = 0; c < BN; c += 64) {  // 64 accumulator columns -> one sub-tile
+        const int b = (c / 64) & 1;
+        if ((BN / 64) % 2 == 1 && c == 0) {
+          if (tid == 0) bulk_wait_group_read<0>();
+          warpgroup_sync(wg);
+        }
 #pragma unroll
-        for (int c = 0; c < BN; c += 64) {
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) {
             const int jr = c / 8 + jj, jg = jr + 4;
@@ -277,101 +316,147 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                 r0 += br.x; r1 += br.y; g0 += bg.x; g1 += bg.y;
               }
             }
-            const int oc = (n0 + c) / 2 + 8 * jj + 2 * q;
-            if (p.epilogue == EPI_GATED_GELU) {
-              *reinterpret_cast<uint32_t*>(out + oc) = pack_bf16(gelu_tanh(r0) * g0, gelu_tanh(r1) * g1);
-            } else {
-              // fp32-accurate mode: exact tanh, result kept to ~16 mantissa bits as [hi | lo | hi]
-              const float v0 = gelu_tanh_exact(r0) * g0, v1 = gelu_tanh_exact(r1) * g1;
-              const uint32_t hi = pack_bf16(v0, v1);
-              const uint32_t lo = pack_bf16(v0 - __bfloat162float(__float2bfloat16_rn(v0)),
-                                            v1 - __bfloat162float(__float2bfloat16_rn(v1)));
-              *reinterpret_cast<uint32_t*>(out + oc) = hi;
-              *reinterpret_cast<uint32_t*>(out + F + oc) = lo;
-              *reinterpret_cast<uint32_t*>(out + 2 * F + oc) = hi;
-            }
+            stg_put(b, h, jj, pack_bf16(gelu_tanh(r0) * g0, gelu_tanh(r1) * g1));
           }
         }
-      } else if (p.epilogue == EPI_BF16) {
-        bf16* out = reinterpret_cast<bf16*>(p.out) + static_cast<size_t>(row) * p.ldo;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int col = n0 + 8 * j + 2 * q;
-          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-          if (p.rs.ss_lo != nullptr) {
-            v0 *= inv_r[h]; v1 *= inv_r[h];
-            if (bias) {
-              const float2 b2 = *reinterpret_cast<const float2*>(cst + 8 * j + 2 * q);
-              v0 += b2.x; v1 += b2.y;
-            }
-          }
-          *reinterpret_cast<uint32_t*>(out + col) = pack_bf16(v0, v1);
+        stg_release();
+        if (tid == 0) {
+          tma_store_2d(&tmap_o, stg + b * STG_BUF_BYTES, (n0 + c) / 2, stg_m);
+          bulk_commit_group();
         }
-      } else if (p.epilogue == EPI_RESID_PREP) {
-        // deferred normalisation, producer side: x = acc + residual (in place), the next GEMM's
-        // operand bf16(x * g) and this tile's share of the row's sum of squares
-        float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
-        bf16* arow = p.prep.a + static_cast<size_t>(row) * p.prep.lda;
-        const float* gvec = row < p.prep.split_row ? cst : cst + BN;
-        float ssum = 0.f;
+      }
+    } else if (p.epilogue == EPI_GATED_GELU_SPLIT3) {
+      // fp32-accurate mode: exact tanh, result kept to ~16 mantissa bits as [hi | lo | hi]: hi in
+      // one buffer, lo in the other, three stores per sub-tile
+      const int F = p.N / 2;
 #pragma unroll
-        for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
-          float2 x[EPI_CHUNK];
+      for (int c = 0; c < BN; c += 64) {
+        if (tid == 0) bulk_wait_group_read<0>();
+        warpgroup_sync(wg);  // both buffers have been read
 #pragma unroll
-          for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-            const int col = n0 + 8 * (j0 + jj) + 2 * q;
-            if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(out + col);
-          }
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-          for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-            const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
-            if (j >= BN / 8) continue;
-            const float v0 = acc[4 * j + 2 * h] + x[jj].x, v1 = acc[4 * j + 2 * h + 1] + x[jj].y;
-            const float2 g = *reinterpret_cast<const float2*>(gvec + 8 * j + 2 * q);
-            ssum = fmaf(v0, v0, ssum);
-            ssum = fmaf(v1, v1, ssum);
-            *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-            *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g.x, v1 * g.y);
+          for (int jj = 0; jj < 4; ++jj) {
+            const int jr = c / 8 + jj, jg = jr + 4;
+            const float r0 = acc[4 * jr + 2 * h], r1 = acc[4 * jr + 2 * h + 1];
+            const float g0 = acc[4 * jg + 2 * h], g1 = acc[4 * jg + 2 * h + 1];
+            const float v0 = gelu_tanh_exact(r0) * g0, v1 = gelu_tanh_exact(r1) * g1;
+            stg_put(0, h, jj, pack_bf16(v0, v1));
+            stg_put(1, h, jj,
+                    pack_bf16(v0 - __bfloat162float(__float2bfloat16_rn(v0)),
+                              v1 - __bfloat162float(__float2bfloat16_rn(v1))));
           }
         }
-        ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
-        ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
-        if (q == 0) p.prep.ss[static_cast<size_t>(n0 / BN) * p.prep.ss_stride + row] = ssum;
-      } else {
-        float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
-        const float* add = nullptr;  // row added to the accumulator
-        if (p.epilogue == EPI_RESID_F32) {
-          add = p.resid + static_cast<size_t>(row) * p.ldo;
-        } else if (p.epilogue == EPI_POS_F32) {
-          const int seq = row / p.pos_rows;
-          int pr = row - seq * p.pos_rows;
-          if (p.pos_shift != nullptr) {
-            pr -= p.pos_shift[seq];
-            if (pr < 0) pr += p.pos_rows;
-          }
-          add = p.pos + static_cast<size_t>(pr) * p.N;
+        stg_release();
+        if (tid == 0) {
+          const int oc = (n0 + c) / 2;
+          tma_store_2d(&tmap_o, stg, oc, stg_m);
+          tma_store_2d(&tmap_o, stg + STG_BUF_BYTES, F + oc, stg_m);
+          tma_store_2d(&tmap_o, stg, 2 * F + oc, stg_m);
+          bulk_commit_group();
         }
-        const bool dup = p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
+      }
+    } else if (p.epilogue == EPI_BF16) {
 #pragma unroll
-        for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
-          float2 x[EPI_CHUNK];
-          if (add != nullptr) {
+      for (int s = 0; s < BN / 32; ++s) {  // an even count: BN is a multiple of 64 here
+        const int b = s & 1;
 #pragma unroll
-            for (int jj = 0; jj < EPI_CHUNK; ++jj)
-              if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(add + n0 + 8 * (j0 + jj) + 2 * q);
-          }
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-          for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-            const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
-            if (j >= BN / 8) continue;
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * s + jj;
             float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            if (add != nullptr) {
-              v0 += x[jj].x; v1 += x[jj].y;
+            if (p.rs.ss_lo != nullptr) {
+              v0 *= inv_r[h]; v1 *= inv_r[h];
+              if (bias) {
+                const float2 b2 = *reinterpret_cast<const float2*>(cst + 8 * j + 2 * q);
+                v0 += b2.x; v1 += b2.y;
+              }
             }
-            *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-            if (dup)
-              *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
-                  make_float2(v0, v1);
+            stg_put(b, h, jj, pack_bf16(v0, v1));
+          }
+        }
+        stg_release();
+        if (tid == 0) {
+          tma_store_2d(&tmap_o, stg + b * STG_BUF_BYTES, n0 + 32 * s, stg_m);
+          bulk_commit_group();
+        }
+      }
+    }
+    // after the CTA's last tile the staged stores must have landed before the grid counts as
+    // complete: dependent kernels read them (only lane 0 of each warpgroup has issued any; for the
+    // others the wait returns at once)
+    if (epi_is_bf16_out(p.epilogue) && tile + static_cast<int>(gridDim.x) >= tiles) bulk_wait_group_all();
+    if (!epi_is_bf16_out(p.epilogue)) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = row_first + 8 * h;
+        if (p.epilogue == EPI_RESID_PREP) {
+          // deferred normalisation, producer side: x = acc + residual (in place), the next GEMM's
+          // operand bf16(x * g) and this tile's share of the row's sum of squares
+          float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
+          bf16* arow = p.prep.a + static_cast<size_t>(row) * p.prep.lda;
+          const float* gvec = row < p.prep.split_row ? cst : cst + BN;
+          float ssum = 0.f;
+#pragma unroll
+          for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
+            float2 x[EPI_CHUNK];
+#pragma unroll
+            for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+              const int col = n0 + 8 * (j0 + jj) + 2 * q;
+              if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(out + col);
+            }
+#pragma unroll
+            for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+              const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+              if (j >= BN / 8) continue;
+              const float v0 = acc[4 * j + 2 * h] + x[jj].x, v1 = acc[4 * j + 2 * h + 1] + x[jj].y;
+              const float2 g = *reinterpret_cast<const float2*>(gvec + 8 * j + 2 * q);
+              ssum = fmaf(v0, v0, ssum);
+              ssum = fmaf(v1, v1, ssum);
+              *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+              *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g.x, v1 * g.y);
+            }
+          }
+          ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
+          ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
+          if (q == 0) p.prep.ss[static_cast<size_t>(n0 / BN) * p.prep.ss_stride + row] = ssum;
+        } else {
+          float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
+          const float* add = nullptr;  // row added to the accumulator
+          if (p.epilogue == EPI_RESID_F32) {
+            add = p.resid + static_cast<size_t>(row) * p.ldo;
+          } else if (p.epilogue == EPI_POS_F32) {
+            const int seq = row / p.pos_rows;
+            int pr = row - seq * p.pos_rows;
+            if (p.pos_shift != nullptr) {
+              pr -= p.pos_shift[seq];
+              if (pr < 0) pr += p.pos_rows;
+            }
+            add = p.pos + static_cast<size_t>(pr) * p.N;
+          }
+          const bool dup = p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
+#pragma unroll
+          for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
+            float2 x[EPI_CHUNK];
+            if (add != nullptr) {
+#pragma unroll
+              for (int jj = 0; jj < EPI_CHUNK; ++jj)
+                if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(add + n0 + 8 * (j0 + jj) + 2 * q);
+            }
+#pragma unroll
+            for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+              const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+              if (j >= BN / 8) continue;
+              float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+              if (add != nullptr) {
+                v0 += x[jj].x; v1 += x[jj].y;
+              }
+              *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+              if (dup)
+                *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
+                    make_float2(v0, v1);
+            }
           }
         }
       }
@@ -407,7 +492,8 @@ static int gemm_sm_count() {
 }
 
 template <int BN>
-int launch_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& d, cudaStream_t st) {
+int launch_bn(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmDev& d,
+              cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
   static_assert(Cfg::SMEM_BYTES <= 227 * 1024 && Cfg::STAGES >= 3, "smem budget");
   const int tiles = (d.N / BN) * (d.M / BLOCK_M);
@@ -417,7 +503,7 @@ int launch_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmDev& d, cu
                  2.0 * (static_cast<double>(d.M) * d.K + static_cast<double>(d.N) * d.K) +
                      4.0 * d.M * d.N, st);
   MSD_CUDA_CHECK(launch_kernel(gemm_bf16_wgmma_kernel<BN>, grid, dim3(GEMM_THREADS), Cfg::SMEM_BYTES,
-                               st, ta, tb, d));
+                               st, ta, tb, to, d));
   ++g_launch_count;
   return 0;
 }
@@ -511,6 +597,14 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   } else if (int rc = make_tmap_bf16_2d(&tb, a.B, a.N, a.K, a.ldb, bn)) {
     return rc;
   }
+  // bf16 outputs are stored by TMA in 64-row x 32-column boxes; the map refuses an output view
+  // whose base is not 16-byte aligned
+  CUtensorMap to;
+  memset(&to, 0, sizeof(to));
+  if (epi_is_bf16_out(a.epilogue)) {
+    const int cols = a.epilogue == EPI_BF16 ? a.N : a.epilogue == EPI_GATED_GELU ? a.N / 2 : 3 * (a.N / 2);
+    if (int rc = make_tmap_bf16_2d(&to, a.out, a.M, cols, a.ldo, 64, 64)) return rc;
+  }
   GemmDev d;
   d.M = a.M; d.N = a.N; d.K = a.K;
   d.epilogue = a.epilogue;
@@ -538,11 +632,11 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
                 "gemm: a step-dependent bias row needs the device step index");
   }
   switch (bn) {
-    case 64: return launch_bn<64>(ta, tb, d, stream);
-    case 96: return launch_bn<96>(ta, tb, d, stream);
-    case 128: return launch_bn<128>(ta, tb, d, stream);
-    case 192: return launch_bn<192>(ta, tb, d, stream);
-    default: return launch_bn<256>(ta, tb, d, stream);
+    case 64: return launch_bn<64>(ta, tb, to, d, stream);
+    case 96: return launch_bn<96>(ta, tb, to, d, stream);
+    case 128: return launch_bn<128>(ta, tb, to, d, stream);
+    case 192: return launch_bn<192>(ta, tb, to, d, stream);
+    default: return launch_bn<256>(ta, tb, to, d, stream);
   }
 }
 

@@ -64,9 +64,10 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
 // TMA tensor maps (driver entry point fetched at run time; no libcuda link).
 // ---------------------------------------------------------------------------
 // 2D row-major bf16 matrix [rows, cols] with leading dimension ld (elements);
-// box = [box_rows, 64 cols] (128-byte inner extent), SWIZZLE_128B.
+// box = [box_rows, 64 cols] (128-byte inner extent), SWIZZLE_128B; with inner_bytes = 64,
+// box = [box_rows, 32 cols], SWIZZLE_64B.
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                      uint64_t ld, uint32_t box_rows);
+                      uint64_t ld, uint32_t box_rows, int inner_bytes = 128);
 
 // ---------------------------------------------------------------------------
 // GEMM: D[M,N] = A[M,K] * B[N,K]^T, bf16 operands (both K-major), fp32 accumulate
