@@ -386,17 +386,14 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
                 "attention: mask words must be 16-byte aligned per row");
   CUtensorMap tq, tk, tv;
   const int width = a.heads * HD;
-  if (a.tmap_q) tq = *a.tmap_q;
-  else if (int rc = make_tmap_bf16_2d(&tq, a.Q, (uint64_t)a.nbatch * a.Lq, width, a.ldq, BQ)) return rc;
+  if (int rc = make_tmap_bf16_2d(&tq, a.Q, (uint64_t)a.nbatch * a.Lq, width, a.ldq, BQ)) return rc;
   const int kv_batch_rows = a.kv_batch_rows > 0 ? a.kv_batch_rows : a.Lk;
   MSD_REQUIRE(a.kv_row0 >= 0 && a.kv_row0 + a.Lk <= kv_batch_rows,
               "attention: key rows [%d, %d) exceed the %d rows per batch", a.kv_row0, a.kv_row0 + a.Lk,
               kv_batch_rows);
   const uint64_t kv_rows = (uint64_t)a.nbatch * kv_batch_rows;
-  if (a.tmap_k) tk = *a.tmap_k;
-  else if (int rc = make_tmap_bf16_2d(&tk, a.K, kv_rows, width, a.ldk, bkv)) return rc;
-  if (a.tmap_v) tv = *a.tmap_v;
-  else if (int rc = make_tmap_bf16_2d(&tv, a.V, kv_rows, width, a.ldv, bkv)) return rc;
+  if (int rc = make_tmap_bf16_2d(&tk, a.K, kv_rows, width, a.ldk, bkv)) return rc;
+  if (int rc = make_tmap_bf16_2d(&tv, a.V, kv_rows, width, a.ldv, bkv)) return rc;
   AttnDev d;
   d.O = a.O; d.ldo = a.ldo; d.heads = a.heads; d.Lq = a.Lq; d.Lk = a.Lk;
   d.mask_bits = a.mask_bits; d.mask_stride_words = a.mask_stride_words;

@@ -97,6 +97,112 @@ __device__ __forceinline__ void warpgroup_sync(int wg) {
   asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
 }
 
+// One consumer warpgroup's two staging buffers of the bf16 outputs, and the thread's place in them:
+// the 16-byte chunk c of local row r sits at chunk c ^ ((r >> 1) & 3) (SWIZZLE_64B), so the 4-byte
+// writes of a warp (8 rows x 4 lanes, one chunk per row) fall on 32 distinct banks.  Bits 4-5 of
+// `thr` hold its row's (r >> 1) & 3, so XOR-ing the chunk into them places it.
+struct Staging {
+  uint8_t* buf;  // buffer b at buf + b * STG_BUF_BYTES
+  uint32_t thr;  // shared address of the thread's first element pair in buffer 0
+  int wg, tid;
+  int count;     // sub-tiles the warpgroup has staged so far, across all of the CTA's tiles
+};
+
+// Drains a tile's bf16 output through the staging buffers, one 64-row x 32-column sub-tile at a
+// time, and moves on without waiting for the global writes.  Sub-tile s: the thread's element pairs
+// pair(s, h, jj) (row h * 8 of its quad's rows, column group jj) go into buffer count & 1, then
+// fence.proxy.async, lane 0 waits until every store issued so far has read its buffer, a warpgroup
+// barrier, and lane 0 stores the buffer at output column cols(s).x (and .y when >= 0) of rows
+// [row, row + 64) and commits the group.  So a buffer is written only after the store that last
+// read it, two sub-tiles earlier in the running count, has been waited for, in whichever tile that
+// was.
+template <int SUBTILES, class Pair, class Cols>
+__device__ __forceinline__ void drain_staged(Staging& st, const CUtensorMap* tmap_o, int row, Pair pair,
+                                             Cols cols) {
+#pragma unroll
+  for (int s = 0; s < SUBTILES; ++s, ++st.count) {
+    const uint32_t b = (st.count & 1) * STG_BUF_BYTES;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) st_shared_u32((st.thr ^ (jj << 4)) + b + h * 8 * 64, pair(s, h, jj));
+    }
+    fence_proxy_async_smem();
+    if (st.tid == 0) bulk_wait_group_read<0>();
+    warpgroup_sync(st.wg);
+    if (st.tid == 0) {
+      const int2 c = cols(s);
+      for (int k = 0; k < (c.y >= 0 ? 2 : 1); ++k) tma_store_2d(tmap_o, st.buf + b, k ? c.y : c.x, row);
+      bulk_commit_group();
+    }
+  }
+}
+
+// Drains a tile's fp32 output (EPI_F32 / EPI_RESID_F32 / EPI_POS_F32, or EPI_RESID_PREP when PREP)
+// straight from the fragment, for the thread's two rows: out = acc + the residual or (rolled)
+// position row, if any, and with EPI_POS_F32 the same again dup_rows rows further down.  PREP, the
+// deferred normalisation's producer side (the residual is the output row, updated in place): also
+// the next GEMM's operand bf16(x * g), with the tile's gains staged at cst, and the tile's share of
+// the row's sum of squares.  Each chunk's EPI_CHUNK row loads are issued ahead of its stores.
+template <int BN, bool PREP>
+__device__ __forceinline__ void drain_f32(const GemmDev& p, const float (&acc)[BN / 2], int row_first,
+                                          int n0, int q, const float* cst) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row_first + 8 * h;
+    float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
+    const float* add = nullptr;  // row added to the accumulator
+    if (PREP || p.epilogue == EPI_RESID_F32) {
+      add = p.resid + static_cast<size_t>(row) * p.ldo;
+    } else if (p.epilogue == EPI_POS_F32) {
+      const int seq = row / p.pos_rows;
+      int pr = row - seq * p.pos_rows;
+      if (p.pos_shift != nullptr) {
+        pr -= p.pos_shift[seq];
+        if (pr < 0) pr += p.pos_rows;
+      }
+      add = p.pos + static_cast<size_t>(pr) * p.N;
+    }
+    const bool dup = !PREP && p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
+    bf16* arow = PREP ? p.prep.a + static_cast<size_t>(row) * p.prep.lda : nullptr;
+    const float* gvec = row < p.prep.split_row ? cst : cst + BN;
+    float ssum = 0.f;
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
+      float2 x[EPI_CHUNK];
+      if (PREP || add != nullptr) {
+#pragma unroll
+        for (int jj = 0; jj < EPI_CHUNK; ++jj)
+          if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(add + n0 + 8 * (j0 + jj) + 2 * q);
+      }
+#pragma unroll
+      for (int jj = 0; jj < EPI_CHUNK; ++jj) {
+        const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+        if (j >= BN / 8) continue;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (PREP || add != nullptr) {
+          v0 += x[jj].x; v1 += x[jj].y;
+        }
+        *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
+        if constexpr (PREP) {
+          const float2 g = *reinterpret_cast<const float2*>(gvec + 8 * j + 2 * q);
+          ssum = fmaf(v0, v0, ssum);
+          ssum = fmaf(v1, v1, ssum);
+          *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g.x, v1 * g.y);
+        }
+        if (dup)
+          *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
+              make_float2(v0, v1);
+      }
+    }
+    if constexpr (PREP) {
+      ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
+      ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
+      if (q == 0) p.prep.ss[static_cast<size_t>(n0 / BN) * p.prep.ss_stride + row] = ssum;
+    }
+  }
+}
+
 // Persistent: gridDim.x CTAs (at most one per SM) walk the 128 x BN output tiles in the static
 // order tile = blockIdx.x + i * gridDim.x, column tiles fastest.  The ring's slot / phase counter
 // runs on across tiles, so the producer streams the next tile's k-blocks while the consumers drain
@@ -199,6 +305,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   } else if (p.rs.ss_lo != nullptr && p.rs.col_bias != nullptr) {
     const0 = p.rs.col_bias + step * p.rs.bias_step_stride;
   }
+  const int stg_row = (warp & 3) * 16 + (lane >> 2);
+  uint8_t* const stg_buf = s_stg + wg * 2 * STG_BUF_BYTES;
+  Staging stg{stg_buf, smem_u32(stg_buf) + stg_row * 64 + (((stg_row >> 1) & 3) << 4) + 4 * q, wg, tid, 0};
   int it = 0;  // k-blocks consumed so far (same count as the producer's)
   for (int tile = blockIdx.x, i = 0; tile < tiles; tile += gridDim.x, ++i) {
     const int n0 = (tile % n_tiles) * BN, m0 = (tile / n_tiles) * BLOCK_M;
@@ -246,220 +355,90 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
 
     // ---------------- epilogue from the accumulator fragment ----------------
     const int row_first = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    // deferred normalisation, consumer side: both rows' scales before the first store, so the
-    // partial-sum loads are in flight together
-    float inv_r[2] = {1.0f, 1.0f};
-    if (p.rs.ss_lo != nullptr) {
-      const float* ssp[2];
-      int parts[2];
+    if (p.epilogue == EPI_RESID_PREP) {
+      drain_f32<BN, true>(p, acc, row_first, n0, q, cst);
+    } else if (!epi_is_bf16_out(p.epilogue)) {
+      drain_f32<BN, false>(p, acc, row_first, n0, q, cst);
+    } else if constexpr (BN % 64 == 0) {  // the launcher refuses width 96 for bf16 outputs
+      // deferred normalisation, consumer side: both rows' scales before the first store, so the
+      // partial-sum loads are in flight together
+      float inv_r[2] = {1.0f, 1.0f};
+      if (p.rs.ss_lo != nullptr) {
+        const float* ssp[2];
+        int parts[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = row_first + 8 * h;
-        const bool lo = row < p.rs.split_row;
-        ssp[h] = (lo ? p.rs.ss_lo : p.rs.ss_hi) + row;
-        parts[h] = lo ? p.rs.parts_lo : p.rs.parts_hi;
-      }
-      float ss[2] = {0.f, 0.f};
-      const int pmax = parts[0] > parts[1] ? parts[0] : parts[1];
+        for (int h = 0; h < 2; ++h) {
+          const int row = row_first + 8 * h;
+          const bool lo = row < p.rs.split_row;
+          ssp[h] = (lo ? p.rs.ss_lo : p.rs.ss_hi) + row;
+          parts[h] = lo ? p.rs.parts_lo : p.rs.parts_hi;
+        }
+        float ss[2] = {0.f, 0.f};
+        const int pmax = parts[0] > parts[1] ? parts[0] : parts[1];
 #pragma unroll 4
-      for (int t = 0; t < pmax; ++t) {
+        for (int t = 0; t < pmax; ++t) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-          if (t < parts[h]) ss[h] += ssp[h][static_cast<size_t>(t) * p.rs.ss_stride];
+          for (int h = 0; h < 2; ++h)
+            if (t < parts[h]) ss[h] += ssp[h][static_cast<size_t>(t) * p.rs.ss_stride];
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) inv_r[h] = rsqrtf(ss[h] * p.rs.inv_d + 1e-6f);
       }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) inv_r[h] = rsqrtf(ss[h] * p.rs.inv_d + 1e-6f);
-    }
-    const bool bias = const0 != nullptr;
-    // bf16 outputs: one 64 x 32 sub-tile at a time into the staging buffer, then lane 0 of the
-    // warpgroup hands it to the TMA unit and the drain moves on without waiting for the global
-    // writes; after the last sub-tile the warpgroup goes straight into the next tile's main loop.
-    // Before the barrier that releases sub-tile k, lane 0 waits until the store of sub-tile k - 1
-    // has read the other buffer, which sub-tile k + 1 overwrites.  Sub-tile s of a tile uses buffer
-    // s & 1; after an odd count the next tile's first sub-tile waits for the last store's read.
-    // this warpgroup's two staging buffers, and the thread's place in them: the 16-byte chunk c of
-    // local row r sits at chunk c ^ ((r >> 1) & 3) (SWIZZLE_64B), so the 4-byte writes of a warp
-    // (8 rows x 4 lanes, one chunk per row) fall on 32 distinct banks.  Bits 4-5 of the thread's
-    // address hold its row's (r >> 1) & 3, so XOR-ing the chunk into them places it.
-    uint8_t* const stg = s_stg + wg * 2 * STG_BUF_BYTES;
-    const int stg_row = (warp & 3) * 16 + (lane >> 2);
-    const uint32_t stg_thr = smem_u32(stg) + stg_row * 64 + (((stg_row >> 1) & 3) << 4) + 4 * q;
-    const int stg_m = m0 + wg * 64;
-    auto stg_put = [&](int b, int h, int jj, uint32_t v) {
-      st_shared_u32((stg_thr ^ (jj << 4)) + b * STG_BUF_BYTES + h * 8 * 64, v);
-    };
-    auto stg_release = [&]() {
-      fence_proxy_async_smem();
-      if (tid == 0) bulk_wait_group_read<0>();
-      warpgroup_sync(wg);
-    };
-    if (p.epilogue == EPI_GATED_GELU) {
-#pragma unroll
-      for (int c = 0; c < BN; c += 64) {  // 64 accumulator columns -> one sub-tile
-        const int b = (c / 64) & 1;
-        if ((BN / 64) % 2 == 1 && c == 0) {
-          if (tid == 0) bulk_wait_group_read<0>();
-          warpgroup_sync(wg);
+      // columns 8 j + 2 q, 8 j + 2 q + 1 of the thread's row h, row-scaled and biased.  Without a
+      // row scale inv_r is 1, which multiplies exactly, so no branch separates the bias loads of
+      // the gated epilogue's two calls
+      auto scaled = [&](int h, int j) {
+        float v0 = acc[4 * j + 2 * h] * inv_r[h], v1 = acc[4 * j + 2 * h + 1] * inv_r[h];
+        if (const0 != nullptr) {
+          const float2 b = *reinterpret_cast<const float2*>(cst + 8 * j + 2 * q);
+          v0 += b.x; v1 += b.y;
         }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int jr = c / 8 + jj, jg = jr + 4;
-            float r0 = acc[4 * jr + 2 * h], r1 = acc[4 * jr + 2 * h + 1];
-            float g0 = acc[4 * jg + 2 * h], g1 = acc[4 * jg + 2 * h + 1];
-            if (p.rs.ss_lo != nullptr) {
-              r0 *= inv_r[h]; r1 *= inv_r[h]; g0 *= inv_r[h]; g1 *= inv_r[h];
-              if (bias) {
-                const float2 br = *reinterpret_cast<const float2*>(cst + 8 * jr + 2 * q);
-                const float2 bg = *reinterpret_cast<const float2*>(cst + 8 * jg + 2 * q);
-                r0 += br.x; r1 += br.y; g0 += bg.x; g1 += bg.y;
-              }
-            }
-            stg_put(b, h, jj, pack_bf16(gelu_tanh(r0) * g0, gelu_tanh(r1) * g1));
-          }
-        }
-        stg_release();
-        if (tid == 0) {
-          tma_store_2d(&tmap_o, stg + b * STG_BUF_BYTES, (n0 + c) / 2, stg_m);
-          bulk_commit_group();
-        }
+        return make_float2(v0, v1);
+      };
+      const int row0 = m0 + wg * 64;
+      if (p.epilogue == EPI_BF16) {
+        drain_staged<BN / 32>(
+            stg, &tmap_o, row0,
+            [&](int s, int h, int jj) {
+              const float2 v = scaled(h, 4 * s + jj);
+              return pack_bf16(v.x, v.y);
+            },
+            [&](int s) { return make_int2(n0 + 32 * s, -1); });
+      } else if (p.epilogue == EPI_GATED_GELU) {
+        // 64 accumulator columns, 32 GELU inputs then their 32 gates, make one sub-tile
+        drain_staged<BN / 64>(
+            stg, &tmap_o, row0,
+            [&](int s, int h, int jj) {
+              const float2 r = scaled(h, 8 * s + jj), g = scaled(h, 8 * s + jj + 4);
+              return pack_bf16(gelu_tanh(r.x) * g.x, gelu_tanh(r.y) * g.y);
+            },
+            [&](int s) { return make_int2(n0 / 2 + 32 * s, -1); });
+      } else {
+        // EPI_GATED_GELU_SPLIT3, the fp32-accurate mode: exact tanh, the result kept to ~16
+        // mantissa bits as [hi | lo | hi], F columns each.  Per 64 accumulator columns, the hi
+        // sub-tile (stored twice), then the lo sub-tile, whose pairs the hi sub-tile computed
+        const int F = p.N / 2;
+        uint32_t lo[2][4] = {};
+        drain_staged<BN / 32>(
+            stg, &tmap_o, row0,
+            [&](int s, int h, int jj) {
+              if (s & 1) return lo[h][jj];
+              const int jr = 8 * (s / 2) + jj, jg = jr + 4;
+              const float v0 = gelu_tanh_exact(acc[4 * jr + 2 * h]) * acc[4 * jg + 2 * h];
+              const float v1 = gelu_tanh_exact(acc[4 * jr + 2 * h + 1]) * acc[4 * jg + 2 * h + 1];
+              lo[h][jj] = pack_bf16(v0 - __bfloat162float(__float2bfloat16_rn(v0)),
+                                    v1 - __bfloat162float(__float2bfloat16_rn(v1)));
+              return pack_bf16(v0, v1);
+            },
+            [&](int s) {
+              const int oc = n0 / 2 + 32 * (s / 2);
+              return s & 1 ? make_int2(F + oc, -1) : make_int2(oc, 2 * F + oc);
+            });
       }
-    } else if (p.epilogue == EPI_GATED_GELU_SPLIT3) {
-      // fp32-accurate mode: exact tanh, result kept to ~16 mantissa bits as [hi | lo | hi]: hi in
-      // one buffer, lo in the other, three stores per sub-tile
-      const int F = p.N / 2;
-#pragma unroll
-      for (int c = 0; c < BN; c += 64) {
-        if (tid == 0) bulk_wait_group_read<0>();
-        warpgroup_sync(wg);  // both buffers have been read
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int jr = c / 8 + jj, jg = jr + 4;
-            const float r0 = acc[4 * jr + 2 * h], r1 = acc[4 * jr + 2 * h + 1];
-            const float g0 = acc[4 * jg + 2 * h], g1 = acc[4 * jg + 2 * h + 1];
-            const float v0 = gelu_tanh_exact(r0) * g0, v1 = gelu_tanh_exact(r1) * g1;
-            stg_put(0, h, jj, pack_bf16(v0, v1));
-            stg_put(1, h, jj,
-                    pack_bf16(v0 - __bfloat162float(__float2bfloat16_rn(v0)),
-                              v1 - __bfloat162float(__float2bfloat16_rn(v1))));
-          }
-        }
-        stg_release();
-        if (tid == 0) {
-          const int oc = (n0 + c) / 2;
-          tma_store_2d(&tmap_o, stg, oc, stg_m);
-          tma_store_2d(&tmap_o, stg + STG_BUF_BYTES, F + oc, stg_m);
-          tma_store_2d(&tmap_o, stg, 2 * F + oc, stg_m);
-          bulk_commit_group();
-        }
-      }
-    } else if (p.epilogue == EPI_BF16) {
-#pragma unroll
-      for (int s = 0; s < BN / 32; ++s) {  // an even count: BN is a multiple of 64 here
-        const int b = s & 1;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * s + jj;
-            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            if (p.rs.ss_lo != nullptr) {
-              v0 *= inv_r[h]; v1 *= inv_r[h];
-              if (bias) {
-                const float2 b2 = *reinterpret_cast<const float2*>(cst + 8 * j + 2 * q);
-                v0 += b2.x; v1 += b2.y;
-              }
-            }
-            stg_put(b, h, jj, pack_bf16(v0, v1));
-          }
-        }
-        stg_release();
-        if (tid == 0) {
-          tma_store_2d(&tmap_o, stg + b * STG_BUF_BYTES, n0 + 32 * s, stg_m);
-          bulk_commit_group();
-        }
-      }
-    }
-    // after the CTA's last tile the staged stores must have landed before the grid counts as
-    // complete: dependent kernels read them (only lane 0 of each warpgroup has issued any; for the
-    // others the wait returns at once)
-    if (epi_is_bf16_out(p.epilogue) && tile + static_cast<int>(gridDim.x) >= tiles) bulk_wait_group_all();
-    if (!epi_is_bf16_out(p.epilogue)) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = row_first + 8 * h;
-        if (p.epilogue == EPI_RESID_PREP) {
-          // deferred normalisation, producer side: x = acc + residual (in place), the next GEMM's
-          // operand bf16(x * g) and this tile's share of the row's sum of squares
-          float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
-          bf16* arow = p.prep.a + static_cast<size_t>(row) * p.prep.lda;
-          const float* gvec = row < p.prep.split_row ? cst : cst + BN;
-          float ssum = 0.f;
-#pragma unroll
-          for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
-            float2 x[EPI_CHUNK];
-#pragma unroll
-            for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-              const int col = n0 + 8 * (j0 + jj) + 2 * q;
-              if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(out + col);
-            }
-#pragma unroll
-            for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-              const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
-              if (j >= BN / 8) continue;
-              const float v0 = acc[4 * j + 2 * h] + x[jj].x, v1 = acc[4 * j + 2 * h + 1] + x[jj].y;
-              const float2 g = *reinterpret_cast<const float2*>(gvec + 8 * j + 2 * q);
-              ssum = fmaf(v0, v0, ssum);
-              ssum = fmaf(v1, v1, ssum);
-              *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-              *reinterpret_cast<uint32_t*>(arow + col) = pack_bf16(v0 * g.x, v1 * g.y);
-            }
-          }
-          ssum += __shfl_xor_sync(0xffffffffu, ssum, 1);
-          ssum += __shfl_xor_sync(0xffffffffu, ssum, 2);
-          if (q == 0) p.prep.ss[static_cast<size_t>(n0 / BN) * p.prep.ss_stride + row] = ssum;
-        } else {
-          float* out = reinterpret_cast<float*>(p.out) + static_cast<size_t>(row) * p.ldo;
-          const float* add = nullptr;  // row added to the accumulator
-          if (p.epilogue == EPI_RESID_F32) {
-            add = p.resid + static_cast<size_t>(row) * p.ldo;
-          } else if (p.epilogue == EPI_POS_F32) {
-            const int seq = row / p.pos_rows;
-            int pr = row - seq * p.pos_rows;
-            if (p.pos_shift != nullptr) {
-              pr -= p.pos_shift[seq];
-              if (pr < 0) pr += p.pos_rows;
-            }
-            add = p.pos + static_cast<size_t>(pr) * p.N;
-          }
-          const bool dup = p.epilogue == EPI_POS_F32 && p.dup_rows > 0;
-#pragma unroll
-          for (int j0 = 0; j0 < BN / 8; j0 += EPI_CHUNK) {
-            float2 x[EPI_CHUNK];
-            if (add != nullptr) {
-#pragma unroll
-              for (int jj = 0; jj < EPI_CHUNK; ++jj)
-                if (j0 + jj < BN / 8) x[jj] = *reinterpret_cast<const float2*>(add + n0 + 8 * (j0 + jj) + 2 * q);
-            }
-#pragma unroll
-            for (int jj = 0; jj < EPI_CHUNK; ++jj) {
-              const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
-              if (j >= BN / 8) continue;
-              float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-              if (add != nullptr) {
-                v0 += x[jj].x; v1 += x[jj].y;
-              }
-              *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
-              if (dup)
-                *reinterpret_cast<float2*>(out + static_cast<size_t>(p.dup_rows) * p.ldo + col) =
-                    make_float2(v0, v1);
-            }
-          }
-        }
-      }
+      // after the CTA's last tile the staged stores must have landed before the grid counts as
+      // complete: dependent kernels read them (only lane 0 of each warpgroup has issued any; for
+      // the others the wait returns at once)
+      if (tile + static_cast<int>(gridDim.x) >= tiles) bulk_wait_group_all();
     }
     if (tracing) {
       const long long t_end = clock64();
@@ -587,16 +566,8 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   MSD_REQUIRE(a.ldo % 8 == 0, "gemm: ldo=%d must be a multiple of 8", a.ldo);
 
   CUtensorMap ta, tb;
-  if (a.tmap_a) {
-    ta = *a.tmap_a;
-  } else if (int rc = make_tmap_bf16_2d(&ta, a.A, a.M, a.K, a.lda, BLOCK_M)) {
-    return rc;
-  }
-  if (a.tmap_b) {
-    tb = *a.tmap_b;
-  } else if (int rc = make_tmap_bf16_2d(&tb, a.B, a.N, a.K, a.ldb, bn)) {
-    return rc;
-  }
+  if (int rc = make_tmap_bf16_2d(&ta, a.A, a.M, a.K, a.lda, BLOCK_M)) return rc;
+  if (int rc = make_tmap_bf16_2d(&tb, a.B, a.N, a.K, a.ldb, bn)) return rc;
   // bf16 outputs are stored by TMA in 64-row x 32-column boxes; the map refuses an output view
   // whose base is not 16-byte aligned
   CUtensorMap to;

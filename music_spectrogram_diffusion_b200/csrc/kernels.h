@@ -128,9 +128,6 @@ struct GemmArgs {
   int pos_rows;
   const int* pos_shift;  // EPI_POS_F32: per (r / pos_rows) roll amount or nullptr
   int dup_rows;          // EPI_POS_F32: also store to row r + dup_rows when > 0
-  // Pre-built tensor maps (engine caches them); when null the launcher builds them.
-  const CUtensorMap* tmap_a;
-  const CUtensorMap* tmap_b;
   int block_n;           // 0 = auto
   int variant;           // tile-width choice: 0 = fewest waves of tiles (default, 96 / 192 allowed),
                          // 1 = power-of-two widths only
@@ -164,7 +161,6 @@ struct AttnArgs {
   bf16* O; int ldo;
   int nbatch, heads, Lq, Lk;
   const uint32_t* mask_bits; int mask_stride_words;
-  const CUtensorMap* tmap_q; const CUtensorMap* tmap_k; const CUtensorMap* tmap_v;
   // split-KV workspace (optional): part_o [attention_workspace_floats(..)] f32, part_ml
   // [rows*heads*max_splits*2] f32; splits 0 = choose automatically (attention_pick_splits),
   // capped by max_splits.
