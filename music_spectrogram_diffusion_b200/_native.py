@@ -19,8 +19,8 @@ _INCLUDE = os.path.join(os.path.dirname(_HERE), 'include')
 LIB_NAME = 'libmsd_b200.so'
 LIB_PATH = os.path.join(_HERE, LIB_NAME)
 SOURCES = ['gemm_wgmma.cu', 'attention_wgmma.cu', 'attention_f32.cu', 'elementwise.cu',
-           'engine.cu', 'audio_mel.cu', 'audio_resample.cu', 'audio_griffin_lim.cu']
-HEADERS = ['common.cuh', 'kernels.h', 'wgmma.cuh', 'audio_fft.cuh', 'philox.cuh']
+           'engine.cu', 'ops.cu', 'audio_mel.cu', 'audio_resample.cu', 'audio_griffin_lim.cu']
+HEADERS = ['common.cuh', 'kernels.h', 'host.h', 'wgmma.cuh', 'audio_fft.cuh', 'philox.cuh']
 NVCC_FLAGS = [
     '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo',
     '-std=c++17', '-Xcompiler', '-fPIC',

@@ -32,6 +32,13 @@ void set_error(const char* fmt, ...);
     }                                                                            \
   } while (0)
 
+// Propagates a non-zero return code (of a launcher or another int-returning helper)
+#define MSD_TRY(expr)                                                            \
+  do {                                                                           \
+    int _rc = (expr);                                                            \
+    if (_rc != 0) return _rc;                                                    \
+  } while (0)
+
 // ----------------------------------------------------------------------------
 // Small device utilities
 // ----------------------------------------------------------------------------

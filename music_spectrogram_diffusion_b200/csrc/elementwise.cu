@@ -8,12 +8,6 @@
 #include "kernels.h"
 #include "philox.cuh"
 
-#define MSD_TRY_RC(expr)      \
-  do {                       \
-    int _rc = (expr);        \
-    if (_rc != 0) return _rc; \
-  } while (0)
-
 namespace msd {
 
 std::atomic<unsigned long long> g_launch_count{0};
@@ -698,7 +692,7 @@ int launch_rmsnorm(const float* x, const float* gamma, int rows, int d, bf16* ou
   p.src_len = 0; p.dst_len = 0; p.dst_off = 0;
   p.ss_out = nullptr; p.gamma_step_stride = 0;
   ProfScope prof(KC_NORM, 0.0, static_cast<double>(rows) * d * (4.0 + (split3 ? 6.0 : 2.0)), stream);
-  MSD_TRY_RC(launch_norm(p, stream));
+  MSD_TRY(launch_norm(p, stream));
   ++g_launch_count;
   return 0;
 }
@@ -714,7 +708,7 @@ int launch_prep_rows(const float* x, const float* g, long long g_step_stride, co
   p.src_len = 0; p.dst_len = 0; p.dst_off = 0;
   p.ss_out = ss_out; p.gamma_step_stride = g_step_stride;
   ProfScope prof(KC_NORM, 0.0, static_cast<double>(rows) * d * 6.0, stream);
-  MSD_TRY_RC(launch_norm(p, stream));
+  MSD_TRY(launch_norm(p, stream));
   ++g_launch_count;
   return 0;
 }
@@ -729,7 +723,7 @@ int launch_rmsnorm_rows_remap(const float* x, const float* gamma, int B, int src
   p.rows = B * src_len; p.d = d; p.ldo = split3 ? 3 * d : d; p.split3 = split3;
   p.src_len = src_len; p.dst_len = dst_len; p.dst_off = dst_off;
   p.ss_out = nullptr; p.gamma_step_stride = 0;
-  MSD_TRY_RC(launch_norm(p, stream));
+  MSD_TRY(launch_norm(p, stream));
   ++g_launch_count;
   return 0;
 }

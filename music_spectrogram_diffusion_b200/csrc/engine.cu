@@ -1,5 +1,7 @@
-// Engine behind the C ABI (include/msd_b200.h): weight repacking, the two encoders, the
-// FiLM-conditioned decoder, the per-step CUDA graph and the 1000-step DDPM loop.
+// Engine behind the C ABI (include/msd_b200.h): the msd_ctx, weight loading and repacking, the
+// conditioning tables, the two encoders, the FiLM-conditioned decoder, the per-step CUDA graph and
+// the 1000-step DDPM loop, and the guidance split over two GPUs.  The entry points that take no
+// msd_ctx (operator hooks, benchmarks, audio operators) are in ops.cu.
 //
 // Reference call stack replaced (SURVEY §3.1):
 //   ContextDiffusionModel.predict_batch_with_aux   msd/models/diffusion/models.py:340-400
@@ -20,12 +22,14 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <vector>
 
 #include "../../include/msd_b200.h"
 #include "common.cuh"
+#include "host.h"
 #include "kernels.h"
 
 namespace msd {
@@ -173,6 +177,8 @@ using namespace msd;
 
 // most column tiles a residual projection can have (narrowest tile: 64 columns of d <= 1024)
 static constexpr size_t kSsParts = 16;
+// most key splits of an attention launch (the split-KV workspace of the cross-attentions)
+static constexpr int kMaxSplits = 12;
 
 struct msd_ctx {
   msd_config cfg;
@@ -308,24 +314,6 @@ struct LinearSchedule {
   }
 };
 
-// Threefry-2x32, 20 rounds (host twin of the device function in elementwise.cu)
-static void threefry2x32_host(uint32_t k0, uint32_t k1, uint32_t x0, uint32_t x1, uint32_t* out) {
-  const uint32_t ks[3] = {k0, k1, k0 ^ k1 ^ 0x1BD11BDAu};
-  static const int rot[2][4] = {{13, 15, 26, 6}, {17, 29, 16, 24}};
-  x0 += ks[0];
-  x1 += ks[1];
-  for (int g = 0; g < 5; ++g) {
-    for (int j = 0; j < 4; ++j) {
-      x0 += x1;
-      x1 = ((x1 << rot[g & 1][j]) | (x1 >> (32 - rot[g & 1][j]))) ^ x0;
-    }
-    x0 += ks[(g + 1) % 3];
-    x1 += ks[(g + 2) % 3] + static_cast<uint32_t>(g + 1);
-  }
-  out[0] = x0;
-  out[1] = x1;
-}
-
 static void build_step_table(const msd_config& c, std::vector<float>& tab) {
   const int n = c.num_steps;
   tab.assign(static_cast<size_t>(n) * MSD_STEP_COLS, 0.f);
@@ -450,12 +438,6 @@ struct Loader {
   }
 };
 
-#define MSD_TRY(expr)        \
-  do {                       \
-    int _rc = (expr);        \
-    if (_rc != 0) return _rc; \
-  } while (0)
-
 static int load_f32(Loader& L, Arena& A, const std::string& name, int64_t s0, int64_t s1,
                     float** out) {
   const msd_tensor* t = L.find(name, s0, s1);
@@ -546,6 +528,71 @@ static int load_encoder(Loader& L, Arena& A, const std::string& name, int layers
   return 0;
 }
 
+// Timestep conditioning tables (network.py:377-394; layers.py:652-666), all fp32: the FiLM table,
+// and in the deferred-normalisation form the column gains and bias rows derived from it
+static int build_conditioning_tables(msd_ctx* c, Loader& L) {
+  Arena& A = c->arena;
+  const msd_config& g = c->cfg;
+  const int d = c->d, steps = g.num_steps, Ld = g.num_decoder_layers;
+  std::vector<float> timing;
+  build_timing_table(g, timing);
+  TempBufs tb;
+  float *d_timing = nullptr, *c1 = nullptr, *c2 = nullptr;
+  MSD_TRY(tb.get(&d_timing, timing.size()));
+  MSD_TRY(tb.get(&c1, static_cast<size_t>(steps) * 4 * d));
+  MSD_TRY(tb.get(&c2, static_cast<size_t>(steps) * 4 * d));
+  MSD_CUDA_CHECK(cudaMemcpyAsync(d_timing, timing.data(), timing.size() * sizeof(float),
+                                 cudaMemcpyHostToDevice, L.st));
+  const msd_tensor* t0 = L.find("decoder/time_emb_dense0/kernel", d, 4 * d);
+  const msd_tensor* t1 = L.find("decoder/time_emb_dense1/kernel", 4 * d, 4 * d);
+  if (!t0 || !t1) return -3;
+  const float* dev = nullptr;
+  MSD_TRY(L.upload(t0, 0, &dev));
+  MSD_TRY(launch_sgemm_f32(d_timing, dev, c1, 4 * d, steps, 4 * d, d, 1, L.st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(L.st));
+  MSD_TRY(L.upload(t1, 0, &dev));
+  MSD_TRY(launch_sgemm_f32(c1, dev, c2, 4 * d, steps, 4 * d, 4 * d, 1, L.st));
+  MSD_CUDA_CHECK(cudaStreamSynchronize(L.st));
+  MSD_TRY(A.alloc(&c->film, static_cast<size_t>(steps) * 2 * Ld * 2 * d));
+  for (int l = 0; l < Ld; ++l) {
+    for (int f = 0; f < 2; ++f) {
+      const std::string nm = "decoder/layers_" + std::to_string(l) + "/FiLMLayer_" +
+                             std::to_string(f) + "/DenseGeneral_0/kernel";
+      const msd_tensor* tf = L.find(nm, 4 * d, 2 * d);
+      if (!tf) return -3;
+      MSD_TRY(L.upload(tf, 0, &dev));
+      float* dst = c->film + static_cast<size_t>(2 * l + f) * 2 * d;
+      MSD_TRY(launch_sgemm_f32(c2, dev, dst, 2 * Ld * 2 * d, steps, 2 * d, 4 * d, 0, L.st));
+      MSD_CUDA_CHECK(cudaStreamSynchronize(L.st));
+    }
+  }
+  if (!c->fused_norm) return 0;
+  // deferred normalisation: per step and layer, the column gains and the FiLM bias rows pushed
+  // through the QKV / wi weights (as the GEMM reads them: packed bf16)
+  const int hh = c->hh, F = c->F;
+  const long long fstride = static_cast<long long>(2) * Ld * 2 * d;
+  MSD_TRY(A.alloc(&c->gtab, static_cast<size_t>(steps) * 2 * Ld * d));
+  MSD_TRY(A.alloc(&c->btab_qkv, static_cast<size_t>(steps) * Ld * 3 * hh));
+  MSD_TRY(A.alloc(&c->btab_wi, static_cast<size_t>(steps) * Ld * 2 * F));
+  for (int l = 0; l < Ld; ++l) {
+    const DecLayer& w = c->dec[l];
+    for (int f = 0; f < 2; ++f) {
+      const float* film = c->film + static_cast<size_t>(2 * l + f) * 2 * d;
+      MSD_TRY(launch_film_gain(film, fstride, f == 0 ? w.ln_self : w.ln_mlp,
+                               c->gtab + static_cast<size_t>(2 * l + f) * d,
+                               static_cast<long long>(2) * Ld * d, steps, d, L.st));
+    }
+    MSD_TRY(launch_film_bias(c->film + static_cast<size_t>(2 * l) * 2 * d + d, fstride, w.self_attn.qkv,
+                             d, c->btab_qkv + static_cast<size_t>(l) * 3 * hh,
+                             static_cast<long long>(Ld) * 3 * hh, steps, 3 * hh, d, L.st));
+    MSD_TRY(launch_film_bias(c->film + static_cast<size_t>(2 * l + 1) * 2 * d + d, fstride, w.mlp.wi, d,
+                             c->btab_wi + static_cast<size_t>(l) * 2 * F,
+                             static_cast<long long>(Ld) * 2 * F, steps, 2 * F, d, L.st));
+  }
+  MSD_CUDA_CHECK(cudaStreamSynchronize(L.st));
+  return 0;
+}
+
 static int load_all(msd_ctx* c, Loader& L) {
   Arena& A = c->arena;
   const msd_config& g = c->cfg;
@@ -586,73 +633,11 @@ static int load_all(msd_ctx* c, Loader& L) {
   MSD_TRY(A.alloc(&c->spec_out, static_cast<size_t>(nd) * 3 * d));
   MSD_TRY(pack_split3(L, "decoder/spec_out_dense/kernel", d, nd, c->spec_out));
 
-  // ---- timestep conditioning tables (network.py:377-394; layers.py:652-666), all fp32
-  const int steps = g.num_steps, Ld = g.num_decoder_layers;
-  std::vector<float> timing;
-  build_timing_table(g, timing);
-  float *d_timing = nullptr, *c1 = nullptr, *c2 = nullptr;
-  MSD_CUDA_CHECK(cudaMalloc(&d_timing, timing.size() * sizeof(float)));
-  MSD_CUDA_CHECK(cudaMalloc(&c1, static_cast<size_t>(steps) * 4 * d * sizeof(float)));
-  MSD_CUDA_CHECK(cudaMalloc(&c2, static_cast<size_t>(steps) * 4 * d * sizeof(float)));
-  int rc = 0;
-  do {
-    if (cudaMemcpyAsync(d_timing, timing.data(), timing.size() * sizeof(float),
-                        cudaMemcpyHostToDevice, L.st) != cudaSuccess) { rc = -2; break; }
-    const msd_tensor* t0 = L.find("decoder/time_emb_dense0/kernel", d, 4 * d);
-    const msd_tensor* t1 = L.find("decoder/time_emb_dense1/kernel", 4 * d, 4 * d);
-    if (!t0 || !t1) { rc = -3; break; }
-    const float* dev = nullptr;
-    if ((rc = L.upload(t0, 0, &dev))) break;
-    if ((rc = launch_sgemm_f32(d_timing, dev, c1, 4 * d, steps, 4 * d, d, 1, L.st))) break;
-    if (cudaStreamSynchronize(L.st) != cudaSuccess) { rc = -2; break; }
-    if ((rc = L.upload(t1, 0, &dev))) break;
-    if ((rc = launch_sgemm_f32(c1, dev, c2, 4 * d, steps, 4 * d, 4 * d, 1, L.st))) break;
-    if (cudaStreamSynchronize(L.st) != cudaSuccess) { rc = -2; break; }
-    if ((rc = A.alloc(&c->film, static_cast<size_t>(steps) * 2 * Ld * 2 * d))) break;
-    for (int l = 0; l < Ld && rc == 0; ++l) {
-      for (int f = 0; f < 2 && rc == 0; ++f) {
-        const std::string nm = "decoder/layers_" + std::to_string(l) + "/FiLMLayer_" +
-                               std::to_string(f) + "/DenseGeneral_0/kernel";
-        const msd_tensor* tf = L.find(nm, 4 * d, 2 * d);
-        if (!tf) { rc = -3; break; }
-        if ((rc = L.upload(tf, 0, &dev))) break;
-        float* dst = c->film + static_cast<size_t>(2 * l + f) * 2 * d;
-        if ((rc = launch_sgemm_f32(c2, dev, dst, 2 * Ld * 2 * d, steps, 2 * d, 4 * d, 0, L.st))) break;
-        if (cudaStreamSynchronize(L.st) != cudaSuccess) { rc = -2; break; }
-      }
-    }
-    if (rc != 0 || !c->fused_norm) break;
-    // deferred normalisation: per step and layer, the column gains and the FiLM bias rows pushed
-    // through the QKV / wi weights (as the GEMM reads them: packed bf16)
-    const int hh = c->hh, F = c->F;
-    const long long fstride = static_cast<long long>(2) * Ld * 2 * d;
-    if ((rc = A.alloc(&c->gtab, static_cast<size_t>(steps) * 2 * Ld * d))) break;
-    if ((rc = A.alloc(&c->btab_qkv, static_cast<size_t>(steps) * Ld * 3 * hh))) break;
-    if ((rc = A.alloc(&c->btab_wi, static_cast<size_t>(steps) * Ld * 2 * F))) break;
-    for (int l = 0; l < Ld && rc == 0; ++l) {
-      const DecLayer& w = c->dec[l];
-      for (int f = 0; f < 2 && rc == 0; ++f) {
-        const float* film = c->film + static_cast<size_t>(2 * l + f) * 2 * d;
-        rc = launch_film_gain(film, fstride, f == 0 ? w.ln_self : w.ln_mlp,
-                              c->gtab + static_cast<size_t>(2 * l + f) * d,
-                              static_cast<long long>(2) * Ld * d, steps, d, L.st);
-      }
-      if (rc == 0)
-        rc = launch_film_bias(c->film + static_cast<size_t>(2 * l) * 2 * d + d, fstride, w.self_attn.qkv,
-                              d, c->btab_qkv + static_cast<size_t>(l) * 3 * hh,
-                              static_cast<long long>(Ld) * 3 * hh, steps, 3 * hh, d, L.st);
-      if (rc == 0)
-        rc = launch_film_bias(c->film + static_cast<size_t>(2 * l + 1) * 2 * d + d, fstride, w.mlp.wi, d,
-                              c->btab_wi + static_cast<size_t>(l) * 2 * F,
-                              static_cast<long long>(Ld) * 2 * F, steps, 2 * F, d, L.st);
-    }
-    if (rc == 0 && cudaStreamSynchronize(L.st) != cudaSuccess) rc = -2;
-  } while (0);
-  cudaFree(d_timing);
-  cudaFree(c1);
-  cudaFree(c2);
-  if (rc == -2) set_error("CUDA error while building conditioning tables: %s",
-                          cudaGetErrorString(cudaGetLastError()));
+  const int rc = build_conditioning_tables(c, L);
+  if (rc == -2) {
+    const std::string why = g_err;
+    set_error("CUDA error while building conditioning tables: %s", why.c_str());
+  }
   return rc;
 }
 
@@ -680,9 +665,6 @@ static int epi_qkv(const msd_ctx* c) { return c->acc ? EPI_F32 : EPI_BF16; }
 static int epi_gated(const msd_ctx* c) { return c->acc ? EPI_GATED_GELU_SPLIT3 : EPI_GATED_GELU; }
 // byte size of an element of the q / k / v / cache buffers
 static size_t qkv_elem(const msd_ctx* c) { return c->acc ? 4 : 2; }
-static const void* at(const msd_ctx* c, const void* base, size_t elems) {
-  return static_cast<const char*>(base) + elems * qkv_elem(c);
-}
 static void* at(const msd_ctx* c, void* base, size_t elems) {
   return static_cast<char*>(base) + elems * qkv_elem(c);
 }
@@ -701,45 +683,24 @@ static int gemm_pos(const bf16* A, int lda, const bf16* B, int ldb, int M, int N
 // Attention over q / k / v views given as (buffer, element offset, leading dimension); the
 // element type follows the mode.  O: the output-projection's input buffer of logical width
 // `o_width` (bf16 [rows, o_width], acc: [rows, 3 * o_width] = [hi | lo | hi]); head h goes to
-// columns o_col + h*64.
-struct AttnExtra {
-  float* part_o = nullptr; float* part_ml = nullptr;
-  int kv_static = 0, kv_batch_rows = 0, kv_row0 = 0;
-};
+// columns o_col + h*64.  `v` brings the split-KV workspace and the K/V row layout, if any.
 static int attention(const msd_ctx* c, const void* Q, size_t qoff, int ldq, const void* K,
                      size_t koff, int ldk, const void* V, size_t voff, int ldv, bf16* O, int o_width,
                      int o_col, int nb, int H, int Lq, int Lk, const uint32_t* bits,
-                     int stride_words, cudaStream_t st, const AttnExtra& x = AttnExtra()) {
-  if (c->acc) {
-    AttnF32Args a;
-    memset(&a, 0, sizeof(a));
-    a.Q = static_cast<const float*>(at(c, Q, qoff)); a.ldq = ldq;
-    a.K = static_cast<const float*>(at(c, K, koff)); a.ldk = ldk;
-    a.V = static_cast<const float*>(at(c, V, voff)); a.ldv = ldv;
-    a.O = O + o_col; a.o_third = o_width;
-    a.nbatch = nb; a.heads = H; a.Lq = Lq; a.Lk = Lk; a.mask_bits = bits;
-    a.mask_stride_words = stride_words; a.kv_batch_rows = x.kv_batch_rows; a.kv_row0 = x.kv_row0;
-    a.part_o = x.part_o; a.part_ml = x.part_ml; a.max_splits = 12;
-    return launch_attention_f32(a, st);
-  }
-  AttnArgs a;
-  memset(&a, 0, sizeof(a));
-  a.kv_static = x.kv_static; a.kv_batch_rows = x.kv_batch_rows; a.kv_row0 = x.kv_row0;
-  a.part_o = x.part_o; a.part_ml = x.part_ml; a.max_splits = 12;
-  {
-    // tuning / test hook: n > 0 forces a tail of n key blocks on every attention of the step that
-    // has more than n blocks of 128 keys (the cross-attentions; the self-attention has 2)
-    const char* f = getenv("MSD_ATTN_TAIL");
-    const int t = f ? atoi(f) : 0;
-    a.tail = (t > 0 && t < Lk / 128) ? t : 0;
-  }
-  a.Q = static_cast<const bf16*>(at(c, Q, qoff)); a.ldq = ldq;
-  a.K = static_cast<const bf16*>(at(c, K, koff)); a.ldk = ldk;
-  a.V = static_cast<const bf16*>(at(c, V, voff)); a.ldv = ldv;
-  a.O = O + o_col; a.ldo = o_width;
-  a.nbatch = nb; a.heads = H; a.Lq = Lq; a.Lk = Lk; a.mask_bits = bits;
-  a.mask_stride_words = stride_words;
-  return launch_attention(a, st);
+                     int stride_words, cudaStream_t st, AttnView v = AttnView()) {
+  v.f32 = c->acc;   // the q / k / v buffers hold fp32 in the fp32-accurate mode
+  v.Q = Q; v.q_off = qoff; v.ldq = ldq;
+  v.K = K; v.k_off = koff; v.ldk = ldk;
+  v.V = V; v.v_off = voff; v.ldv = ldv;
+  v.O = O + o_col; v.ldo = o_width;
+  v.nbatch = nb; v.heads = H; v.Lq = Lq; v.Lk = Lk;
+  v.mask_bits = bits; v.mask_stride_words = stride_words;
+  v.max_splits = kMaxSplits;
+  // tuning / test hook: n > 0 forces a tail of n key blocks on every attention of the step that
+  // has more than n blocks of 128 keys (the cross-attentions; the self-attention has 2)
+  const int t = attn_switches().tail;
+  v.tail = (t > 0 && t < Lk / 128) ? t : 0;
+  return launch_attention_view(v, st);
 }
 
 // rmsnorm (+FiLM) into a GEMM-input buffer of logical width d
@@ -779,7 +740,7 @@ static int run_encoder(msd_ctx* c, const Encoder& e, int B, int len, const uint3
 static int cross_attention(const msd_ctx* c, int l, int nseg, bf16* o, cudaStream_t st) {
   const int hh = c->hh, N = c->N, words = c->Mkv / 32;
   const size_t kv = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;  // elements
-  AttnExtra ex;
+  AttnView ex = {};
   ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml;
   ex.kv_static = 1;
   if (c->cfg.cross_attend_style == 0)
@@ -1054,18 +1015,6 @@ static void drop_graph(msd_ctx* c) {
   c->graph_batch = -1;
 }
 
-struct TempBufs {
-  std::vector<void*> p;
-  ~TempBufs() { for (void* q : p) cudaFree(q); }
-  template <typename T> int get(T** out, size_t n) {
-    void* q = nullptr;
-    MSD_CUDA_CHECK(cudaMalloc(&q, (n ? n : 1) * sizeof(T)));
-    p.push_back(q);
-    *out = reinterpret_cast<T*>(q);
-    return 0;
-  }
-};
-
 }  // namespace msd
 
 // ===========================================================================
@@ -1091,7 +1040,8 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   MSD_TRY(gemm_configure());
   MSD_TRY(attention_configure());
   MSD_TRY(elementwise_configure());
-  msd_ctx* c = new msd_ctx();
+  // destroys the context on every early return below
+  std::unique_ptr<msd_ctx, void (*)(msd_ctx*)> c(new msd_ctx(), msd_destroy);
   c->cfg = *cfg;
   c->device = device;
   c->d = cfg->emb_dim; c->H = cfg->num_heads; c->hh = cfg->num_heads * 64; c->F = cfg->mlp_dim;
@@ -1106,105 +1056,76 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   const size_t R = static_cast<size_t>(c->passes) * c->Bmax * c->N;
   const size_t BN = static_cast<size_t>(c->Bmax) * c->N;
   const size_t ER = static_cast<size_t>(c->Bmax) * (c->T > c->C ? c->T : c->C);
-  int rc = 0;
-  do {
-    {
-      // Opt-in experiment (MSD_TWO_STREAMS=1): conditional / unconditional passes as two concurrent
-      // kernel chains.  Every GEMM / attention CTA owns a whole SM's shared memory, so the chains
-      // mostly time-share SMs, and the half-height GEMMs are less efficient -> off by default.
-      const char* ts = getenv("MSD_TWO_STREAMS");
-      c->two_streams = (ts && ts[0] == '1') && !c->acc;
-    }
-    if (cudaStreamCreateWithFlags(&c->work, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&c->work2, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_in, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_out, cudaEventDisableTiming) != cudaSuccess) {
-      set_error("msd_create: stream/event creation failed");
-      rc = -2;
-      break;
-    }
-    if ((rc = A.alloc(&c->x, R * c->d))) break;
-    if ((rc = A.alloc(&c->xn, R * 3 * c->d))) break;
-    if ((rc = A.alloc(&c->qkv, R * 3 * c->hh * qe))) break;
-    if ((rc = A.alloc(&c->attn, R * c->hh * ks))) break;
-    if ((rc = A.alloc(&c->hmid, R * c->F * ks))) break;
-    if ((rc = A.alloc(&c->qc, BN * c->hh * (cfg->cross_attend_style == 1 ? 2 : 1) * qe))) break;
-    if (cfg->cross_attend_style == 1 && (rc = A.alloc(&c->attn2, BN * 2 * c->hh * ks))) break;
-    constexpr int kMaxSplits = 12;
-    const size_t npart = attention_workspace_floats(c->Bmax, c->H, c->N, kMaxSplits);
-    if ((rc = A.alloc(&c->attn_part_o, npart))) break;
-    if ((rc = A.alloc(&c->attn_part_ml, BN * c->H * kMaxSplits * 2))) break;
-    c->attn_part_o2 = c->attn_part_o; c->attn_part_ml2 = c->attn_part_ml;
-    if (cfg->cross_attend_style == 1) {
-      if ((rc = A.alloc(&c->attn_part_o2, npart))) break;
-      if ((rc = A.alloc(&c->attn_part_ml2, BN * c->H * kMaxSplits * 2))) break;
-    }
-    {
-      // MSD_FUSED_NORM=0: tuning / test hook, keeps the stand-alone rmsnorm kernels
-      const char* fn = getenv("MSD_FUSED_NORM");
-      c->fused_norm = !c->acc && !c->two_streams && !(fn && fn[0] == '0');
-      if (c->fused_norm) {
-        if ((rc = A.alloc(&c->ss_x, kSsParts * R))) break;
-        if ((rc = A.alloc(&c->ss_so, kSsParts * R))) break;
-        if ((rc = A.alloc(&c->ss_co, kSsParts * R))) break;
-      }
-    }
-    if ((rc = A.alloc(&c->eps, R * c->nd))) break;
-    if ((rc = A.alloc(&c->z, BN * c->nd))) break;
-    if ((rc = A.alloc(&c->z_split, BN * 3 * c->nd))) break;
-    if ((rc = A.alloc(&c->kv_cache, static_cast<size_t>(cfg->num_decoder_layers) * c->Bmax *
-                                        c->Mkv * 2 * c->hh * qe))) break;
-    if ((rc = A.alloc(&c->enc, static_cast<size_t>(c->Bmax) * c->Mkv * c->d * ks))) break;
-    if ((rc = A.alloc(&c->ex, ER * c->d))) break;
-    if ((rc = A.alloc(&c->exn, ER * c->d * ks))) break;
-    if ((rc = A.alloc(&c->eqkv, ER * 3 * c->hh * qe))) break;
-    if ((rc = A.alloc(&c->eattn, ER * c->hh * ks))) break;
-    if ((rc = A.alloc(&c->eh, ER * c->F * ks))) break;
-    if ((rc = A.alloc(&c->ctx_split, static_cast<size_t>(c->Bmax) * c->C * 3 * c->nd))) break;
-    if ((rc = A.alloc(&c->mask_bits, static_cast<size_t>(c->Bmax) * (c->Mkv / 32)))) break;
-    if ((rc = A.alloc(&c->ctx_seq_len, static_cast<size_t>(c->Bmax)))) break;
-    if ((rc = A.alloc(&c->run, 1))) break;
-    if (cudaMemset(c->run, 0, sizeof(RunArgs)) != cudaSuccess) {
-      set_error("msd_create: cudaMemset failed");
-      rc = -2;
-      break;
-    }
-    c->d_step = &c->run->step;
-    {
-      const size_t xf = 2 * BN * c->nd + 64;
-      if ((rc = A.alloc(&c->xchg, xf))) break;
-      if (cudaMemset(c->xchg, 0, xf * sizeof(float)) != cudaSuccess) {
-        set_error("msd_create: cudaMemset failed");
-        rc = -2;
-        break;
-      }
-    }
-    if ((rc = A.alloc(&c->coef, static_cast<size_t>(cfg->num_steps) * MSD_STEP_COLS))) break;
-    if ((rc = A.alloc(&c->rng_keys, (static_cast<size_t>(cfg->num_steps) + 1) * 2))) break;
-    if (cudaMemset(c->rng_keys, 0, (static_cast<size_t>(cfg->num_steps) + 1) * 2 * sizeof(uint32_t)) !=
-        cudaSuccess) {
-      set_error("msd_create: cudaMemset failed");
-      rc = -2;
-      break;
-    }
-    if ((rc = A.alloc(&c->row_keys, static_cast<size_t>(c->Bmax) * (cfg->num_steps + 1) * 2))) break;
-    if ((rc = A.alloc(&c->row_seeds, static_cast<size_t>(c->Bmax)))) break;
-    c->row_seeds_host.assign(c->Bmax, 0ull);
-    c->row_keys_valid.assign(c->Bmax, 0);
-    build_step_table(*cfg, c->coef_host);
-    if (cudaMemcpy(c->coef, c->coef_host.data(), c->coef_host.size() * sizeof(float),
-                   cudaMemcpyHostToDevice) != cudaSuccess) {
-      set_error("msd_create: coefficient upload failed");
-      rc = -2;
-    }
-  } while (0);
-  if (rc != 0) {
-    msd_destroy(c);
-    return rc;
+  {
+    // Opt-in experiment (MSD_TWO_STREAMS=1): conditional / unconditional passes as two concurrent
+    // kernel chains.  Every GEMM / attention CTA owns a whole SM's shared memory, so the chains
+    // mostly time-share SMs, and the half-height GEMMs are less efficient -> off by default.
+    const char* ts = getenv("MSD_TWO_STREAMS");
+    c->two_streams = (ts && ts[0] == '1') && !c->acc;
   }
-  *out = c;
+  MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&c->work, cudaStreamNonBlocking));
+  MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&c->work2, cudaStreamNonBlocking));
+  MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
+  MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
+  MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_in, cudaEventDisableTiming));
+  MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_out, cudaEventDisableTiming));
+  MSD_TRY(A.alloc(&c->x, R * c->d));
+  MSD_TRY(A.alloc(&c->xn, R * 3 * c->d));
+  MSD_TRY(A.alloc(&c->qkv, R * 3 * c->hh * qe));
+  MSD_TRY(A.alloc(&c->attn, R * c->hh * ks));
+  MSD_TRY(A.alloc(&c->hmid, R * c->F * ks));
+  MSD_TRY(A.alloc(&c->qc, BN * c->hh * (cfg->cross_attend_style == 1 ? 2 : 1) * qe));
+  if (cfg->cross_attend_style == 1) MSD_TRY(A.alloc(&c->attn2, BN * 2 * c->hh * ks));
+  const size_t npart = attention_workspace_floats(c->Bmax, c->H, c->N, kMaxSplits);
+  MSD_TRY(A.alloc(&c->attn_part_o, npart));
+  MSD_TRY(A.alloc(&c->attn_part_ml, BN * c->H * kMaxSplits * 2));
+  c->attn_part_o2 = c->attn_part_o; c->attn_part_ml2 = c->attn_part_ml;
+  if (cfg->cross_attend_style == 1) {
+    MSD_TRY(A.alloc(&c->attn_part_o2, npart));
+    MSD_TRY(A.alloc(&c->attn_part_ml2, BN * c->H * kMaxSplits * 2));
+  }
+  {
+    // MSD_FUSED_NORM=0: tuning / test hook, keeps the stand-alone rmsnorm kernels
+    const char* fn = getenv("MSD_FUSED_NORM");
+    c->fused_norm = !c->acc && !c->two_streams && !(fn && fn[0] == '0');
+    if (c->fused_norm) {
+      MSD_TRY(A.alloc(&c->ss_x, kSsParts * R));
+      MSD_TRY(A.alloc(&c->ss_so, kSsParts * R));
+      MSD_TRY(A.alloc(&c->ss_co, kSsParts * R));
+    }
+  }
+  MSD_TRY(A.alloc(&c->eps, R * c->nd));
+  MSD_TRY(A.alloc(&c->z, BN * c->nd));
+  MSD_TRY(A.alloc(&c->z_split, BN * 3 * c->nd));
+  MSD_TRY(A.alloc(&c->kv_cache, static_cast<size_t>(cfg->num_decoder_layers) * c->Bmax *
+                                    c->Mkv * 2 * c->hh * qe));
+  MSD_TRY(A.alloc(&c->enc, static_cast<size_t>(c->Bmax) * c->Mkv * c->d * ks));
+  MSD_TRY(A.alloc(&c->ex, ER * c->d));
+  MSD_TRY(A.alloc(&c->exn, ER * c->d * ks));
+  MSD_TRY(A.alloc(&c->eqkv, ER * 3 * c->hh * qe));
+  MSD_TRY(A.alloc(&c->eattn, ER * c->hh * ks));
+  MSD_TRY(A.alloc(&c->eh, ER * c->F * ks));
+  MSD_TRY(A.alloc(&c->ctx_split, static_cast<size_t>(c->Bmax) * c->C * 3 * c->nd));
+  MSD_TRY(A.alloc(&c->mask_bits, static_cast<size_t>(c->Bmax) * (c->Mkv / 32)));
+  MSD_TRY(A.alloc(&c->ctx_seq_len, static_cast<size_t>(c->Bmax)));
+  MSD_TRY(A.alloc(&c->run, 1));
+  MSD_CUDA_CHECK(cudaMemset(c->run, 0, sizeof(RunArgs)));
+  c->d_step = &c->run->step;
+  const size_t xf = 2 * BN * c->nd + 64;
+  MSD_TRY(A.alloc(&c->xchg, xf));
+  MSD_CUDA_CHECK(cudaMemset(c->xchg, 0, xf * sizeof(float)));
+  MSD_TRY(A.alloc(&c->coef, static_cast<size_t>(cfg->num_steps) * MSD_STEP_COLS));
+  MSD_TRY(A.alloc(&c->rng_keys, (static_cast<size_t>(cfg->num_steps) + 1) * 2));
+  MSD_CUDA_CHECK(cudaMemset(c->rng_keys, 0,
+                            (static_cast<size_t>(cfg->num_steps) + 1) * 2 * sizeof(uint32_t)));
+  MSD_TRY(A.alloc(&c->row_keys, static_cast<size_t>(c->Bmax) * (cfg->num_steps + 1) * 2));
+  MSD_TRY(A.alloc(&c->row_seeds, static_cast<size_t>(c->Bmax)));
+  c->row_seeds_host.assign(c->Bmax, 0ull);
+  c->row_keys_valid.assign(c->Bmax, 0);
+  build_step_table(*cfg, c->coef_host);
+  MSD_CUDA_CHECK(cudaMemcpy(c->coef, c->coef_host.data(), c->coef_host.size() * sizeof(float),
+                            cudaMemcpyHostToDevice));
+  *out = c.release();
   return 0;
 }
 
@@ -1241,22 +1162,15 @@ int msd_load_weights(msd_ctx* c, const msd_tensor* tensors, int32_t n) {
   L.stage_elems = biggest;
   L.st = c->work;
   L.ks = c->ks;
-  MSD_CUDA_CHECK(cudaMalloc(&L.stage, biggest * sizeof(float)));
-  if (cudaMalloc(&L.stage2, biggest * sizeof(float)) != cudaSuccess) {
-    cudaFree(L.stage);
-    set_error("msd_load_weights: staging allocation failed");
-    return -2;
-  }
-  int rc = load_all(c, L);
-  cudaError_t e = cudaStreamSynchronize(c->work);
-  cudaFree(L.stage);
-  cudaFree(L.stage2);
-  if (rc == 0 && e != cudaSuccess) {
-    set_error("msd_load_weights: %s", cudaGetErrorString(e));
-    rc = -2;
-  }
-  if (rc == 0) c->weights_loaded = true;
-  return rc;
+  TempBufs staging;
+  MSD_TRY(staging.get(&L.stage, biggest));
+  MSD_TRY(staging.get(&L.stage2, biggest));
+  const int rc = load_all(c, L);
+  const cudaError_t e = cudaStreamSynchronize(c->work);  // before the staging buffers are freed
+  MSD_TRY(rc);
+  MSD_CUDA_CHECK(e);
+  c->weights_loaded = true;
+  return 0;
 }
 
 static int begin_on(msd_ctx* c, cudaStream_t caller) {
@@ -1420,10 +1334,7 @@ int msd_sample(msd_ctx* c, const float* init_z, const float* noise, uint64_t see
     // PRNGKey(seed) and fold_in(key, i) for every scan index (host threefry, 8 KB upload); the
     // captured step graph reads the table, so a new seed does not force a re-capture
     std::vector<uint32_t> keys(2 * (static_cast<size_t>(steps) + 1));
-    keys[0] = static_cast<uint32_t>(seed >> 32);
-    keys[1] = static_cast<uint32_t>(seed);
-    for (int i = 0; i < steps; ++i)
-      threefry2x32_host(keys[0], keys[1], 0u, static_cast<uint32_t>(i), &keys[2 * (i + 1)]);
+    step_keys(seed, steps, keys.data());
     MSD_CUDA_CHECK(cudaMemcpyAsync(c->rng_keys, keys.data(), keys.size() * sizeof(uint32_t),
                                    cudaMemcpyHostToDevice, st));
     MSD_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -1460,10 +1371,7 @@ int msd_sample_rows(msd_ctx* c, const uint64_t* seeds, float* mel_out, void* str
     c->row_keys_valid[b] = 0;  // until the upload below has completed
     if (c->cfg.rng_kind != 1) continue;
     uint32_t* k = keys.data() + b * stride;
-    k[0] = static_cast<uint32_t>(seeds[b] >> 32);
-    k[1] = static_cast<uint32_t>(seeds[b]);
-    for (int i = 0; i < steps; ++i)
-      threefry2x32_host(k[0], k[1], 0u, static_cast<uint32_t>(i), &k[2 * (i + 1)]);
+    step_keys(seeds[b], steps, k);
     MSD_CUDA_CHECK(cudaMemcpyAsync(c->row_keys + b * stride, k, stride * sizeof(uint32_t),
                                    cudaMemcpyHostToDevice, st));
   }
@@ -1562,724 +1470,6 @@ int msd_profile_step(msd_ctx* c, int32_t step_i, int32_t reps, double* out) {
   return 0;
 }
 
-// ---------------------------------------------------------------------------
-// operator-level entry points
-// ---------------------------------------------------------------------------
-int msd_op_dense(const float* a, const float* w, int32_t M, int32_t N, int32_t K, float* out,
-                 void* stream) {
-  return msd_op_dense_variant(a, w, M, N, K, out, 0, 0, stream);
-}
-
-int msd_op_dense_variant(const float* a, const float* w, int32_t M, int32_t N, int32_t K,
-                         float* out, int32_t variant, int32_t block_n, void* stream) {
-  MSD_REQUIRE(a && w && out, "msd_op_dense: null argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  TempBufs tb;
-  bf16 *ab = nullptr, *wb = nullptr;
-  MSD_TRY(tb.get(&ab, static_cast<size_t>(M) * K));
-  MSD_TRY(tb.get(&wb, static_cast<size_t>(N) * K));
-  MSD_TRY(launch_f32_to_bf16(a, ab, static_cast<long long>(M) * K, st));
-  MSD_TRY(launch_pack_weight(w, K, N, wb, K, 0, 0, 0, st));
-  GemmArgs ga;
-  memset(&ga, 0, sizeof(ga));
-  ga.A = ab; ga.B = wb; ga.M = M; ga.N = N; ga.K = K; ga.lda = K; ga.ldb = K;
-  ga.epilogue = EPI_F32; ga.out = out; ga.ldo = N; ga.variant = variant; ga.block_n = block_n;
-  MSD_TRY(launch_gemm(ga, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t variant,
-                   int32_t block_n, int32_t iters, float* ms_out) {
-  MSD_REQUIRE(ms_out && iters > 0, "msd_bench_gemm: bad argument");
-  TempBufs tb;
-  bf16 *a = nullptr, *b = nullptr;
-  float *o = nullptr, *r = nullptr;
-  MSD_TRY(tb.get(&a, static_cast<size_t>(M) * K));
-  MSD_TRY(tb.get(&b, static_cast<size_t>(N) * K));
-  MSD_TRY(tb.get(&o, static_cast<size_t>(M) * N));
-  MSD_TRY(tb.get(&r, static_cast<size_t>(M) * N));
-  MSD_CUDA_CHECK(cudaMemset(a, 0, static_cast<size_t>(M) * K * 2));
-  MSD_CUDA_CHECK(cudaMemset(b, 0, static_cast<size_t>(N) * K * 2));
-  MSD_CUDA_CHECK(cudaMemset(r, 0, static_cast<size_t>(M) * N * 4));
-  GemmArgs ga;
-  memset(&ga, 0, sizeof(ga));
-  ga.A = a; ga.B = b; ga.M = M; ga.N = N; ga.K = K; ga.lda = K; ga.ldb = K;
-  ga.epilogue = epilogue; ga.out = o; ga.ldo = (epilogue == EPI_GATED_GELU) ? N / 2 : N;
-  ga.resid = (variant == 1) ? r : o;  // default variant: in place, like the engine
-  ga.variant = variant; ga.block_n = block_n;
-  const bool trace = getenv("MSD_GEMM_TRACE") != nullptr;
-  if (trace && (epilogue == EPI_BF16 || epilogue == EPI_GATED_GELU)) {
-    // traced like the decoder's QKV / cross-q / wi launches: a row scale from one partial sum per
-    // row and a bias row (zero-filled tables)
-    float *ss = nullptr, *bias = nullptr;
-    MSD_TRY(tb.get(&ss, static_cast<size_t>(M)));
-    MSD_TRY(tb.get(&bias, static_cast<size_t>(N)));
-    MSD_CUDA_CHECK(cudaMemset(ss, 0, static_cast<size_t>(M) * 4));
-    MSD_CUDA_CHECK(cudaMemset(bias, 0, static_cast<size_t>(N) * 4));
-    ga.rs.ss_lo = ss; ga.rs.ss_hi = ss; ga.rs.parts_lo = 1; ga.rs.parts_hi = 1;
-    ga.rs.split_row = M; ga.rs.ss_stride = M; ga.rs.inv_d = 1.0f / static_cast<float>(K);
-    ga.rs.col_bias = bias;
-  }
-  cudaStream_t st = nullptr;
-  MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0);
-  cudaEventCreate(&e1);
-  int rc = 0;
-  for (int i = 0; i < 3 && rc == 0; ++i) rc = launch_gemm(ga, st);
-  cudaEventRecord(e0, st);
-  for (int i = 0; i < iters && rc == 0; ++i) rc = launch_gemm(ga, st);
-  cudaEventRecord(e1, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  *ms_out = ms / iters;
-  if (trace && variant != 1 && rc == 0 && e == cudaSuccess) {
-    // one more launch with per-tile stamps (after a warm one right before it, like in the loop)
-    long long* tr = nullptr;
-    if (tb.get(&tr, 8 * 512) == 0) {
-      cudaMemsetAsync(tr, 0, 8 * 512 * sizeof(long long), st);
-      launch_gemm(ga, st);
-      ga.trace = tr;
-      // without the programmatic dependency the traced launch starts after the warm one has
-      // finished, so its main loop does not include waiting for that launch's tail
-      g_pdl_skip_next = true;
-      launch_gemm(ga, st);
-      ga.trace = nullptr;
-      std::vector<long long> h(8 * 512);
-      cudaStreamSynchronize(st);
-      cudaMemcpy(h.data(), tr, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-      long long t0 = 0, t1 = 0;
-      int n = 0;
-      double sum[4] = {0, 0, 0, 0};
-      for (int b = 0; b < 512; ++b) {
-        const long long* r = &h[b * 8];
-        if (r[1] == 0) continue;
-        if (n == 0 || r[1] < t0) t0 = r[1];
-        if (n == 0 || r[2] > t1) t1 = r[2];
-        // r[3] = cycles in the tile; r[4..7] clock64 offsets from its start
-        sum[0] += static_cast<double>(r[3]);
-        sum[1] += static_cast<double>(r[4]);
-        sum[2] += static_cast<double>(r[6] - r[5]);
-        sum[3] += static_cast<double>(r[7] - r[6]);
-        ++n;
-      }
-      const double inv_n = n ? 1.0 / n : 0.0;
-      fprintf(stderr, "[gemm trace] M=%d N=%d K=%d epi=%d block_n=%d (automatic %d): %d tiles, first start -> "
-              "last end %.2f us, mean cycles per tile %.0f: set-up %.0f, main loop %.0f (%.0f per k-block), "
-              "epilogue %.0f\n", M, N, K, epilogue, gemm_resolve_block_n(ga), gemm_pick_wide_bn(M, N, epilogue), n,
-              (t1 - t0) * 1e-3, sum[0] * inv_n, sum[1] * inv_n, sum[2] * inv_n, sum[2] * inv_n / (K / 64),
-              sum[3] * inv_n);
-      for (int b = 0; b < 4 && b < 512; ++b) {
-        const long long* r = &h[b * 8];
-        if (r[1] == 0) continue;
-        fprintf(stderr, "[gemm trace]   tile %d sm %lld: start +%.2f us, end +%.2f us; cycles: total %lld, "
-                "setup->wait %lld, wait->acc %lld, acc->stored %lld\n", b, r[0], (r[1] - t0) * 1e-3,
-                (r[2] - t0) * 1e-3, r[3], r[5] - r[4], r[6] - r[5], r[7] - r[6]);
-      }
-      // the tiles of CTA 0 in order: main loop, drain (bf16 outputs: until the last sub-tile is
-      // handed to TMA, whose global writes then run under the next tile's main loop)
-      int sms = 0;
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
-      const int grid = std::min(n, sms > 0 ? sms : n);
-      for (int b = 0, i = 0; grid > 0 && b < 512; b += grid, ++i) {
-        const long long* r = &h[b * 8];
-        if (r[1] == 0) break;
-        fprintf(stderr, "[gemm trace]   CTA 0 tile %d (#%d): start +%.2f us; cycles: main loop %lld, drain %lld\n",
-                i, b, (r[1] - t0) * 1e-3, r[6] - r[5], r[7] - r[6]);
-      }
-    }
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  cudaStreamDestroy(st);
-  if (rc != 0) return rc;
-  MSD_CUDA_CHECK(e);
-  return 0;
-}
-
-int msd_bench_attention(int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32_t iters,
-                        float* ms_out) {
-  MSD_REQUIRE(ms_out && iters > 0, "msd_bench_attention: bad argument");
-  const int w = heads * 64;
-  TempBufs tb;
-  bf16 *qb, *kb, *vb, *ob;
-  float *tmp, *po, *pml;
-  const size_t nq = static_cast<size_t>(nb) * Lq * w, nk = static_cast<size_t>(nb) * Lk * w;
-  MSD_TRY(tb.get(&qb, nq)); MSD_TRY(tb.get(&kb, nk)); MSD_TRY(tb.get(&vb, nk)); MSD_TRY(tb.get(&ob, nq));
-  MSD_TRY(tb.get(&tmp, nk));
-  MSD_TRY(tb.get(&po, attention_workspace_floats(nb, heads, Lq, 12)));
-  MSD_TRY(tb.get(&pml, static_cast<size_t>(nb) * Lq * heads * 12 * 2));
-  cudaStream_t st = nullptr;
-  MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  // N(0,1) * 0.3-ish values through the jax generator (any bounded values would do)
-  MSD_TRY(launch_jax_normal(1u, 2u, static_cast<long long>(nk), tmp, st));
-  MSD_TRY(launch_f32_to_bf16(tmp, kb, static_cast<long long>(nk), st));
-  MSD_TRY(launch_f32_to_bf16(tmp, vb, static_cast<long long>(nk), st));
-  MSD_TRY(launch_f32_to_bf16(tmp, qb, static_cast<long long>(nq), st));
-  AttnArgs aa;
-  memset(&aa, 0, sizeof(aa));
-  aa.Q = qb; aa.ldq = w; aa.K = kb; aa.ldk = w; aa.V = vb; aa.ldv = w; aa.O = ob; aa.ldo = w;
-  aa.nbatch = nb; aa.heads = heads; aa.Lq = Lq; aa.Lk = Lk;
-  aa.part_o = po; aa.part_ml = pml; aa.max_splits = 12; aa.kv_static = 1;
-  {
-    const char* f = getenv("MSD_ATTN_SPLITS");
-    aa.splits = f ? atoi(f) : 0;
-    const char* t = getenv("MSD_ATTN_TAIL");
-    aa.tail = t ? atoi(t) : 0;
-  }
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0);
-  cudaEventCreate(&e1);
-  int rc = 0;
-  for (int i = 0; i < 3 && rc == 0; ++i) rc = launch_attention(aa, st);
-  cudaEventRecord(e0, st);
-  for (int i = 0; i < iters && rc == 0; ++i) rc = launch_attention(aa, st);
-  cudaEventRecord(e1, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  *ms_out = ms / iters;
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  cudaStreamDestroy(st);
-  if (rc != 0) return rc;
-  MSD_CUDA_CHECK(e);
-  return 0;
-}
-
-int msd_op_attention(const float* q, const float* k, const float* v, const int32_t* key_mask,
-                     int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, float* out, void* stream) {
-  MSD_REQUIRE(q && k && v && out, "msd_op_attention: null argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int w = heads * 64;
-  TempBufs tb;
-  bf16 *qb, *kb, *vb, *ob;
-  uint32_t* bits = nullptr;
-  MSD_TRY(tb.get(&qb, static_cast<size_t>(nb) * Lq * w));
-  MSD_TRY(tb.get(&kb, static_cast<size_t>(nb) * Lk * w));
-  MSD_TRY(tb.get(&vb, static_cast<size_t>(nb) * Lk * w));
-  MSD_TRY(tb.get(&ob, static_cast<size_t>(nb) * Lq * w));
-  MSD_TRY(launch_f32_to_bf16(q, qb, static_cast<long long>(nb) * Lq * w, st));
-  MSD_TRY(launch_f32_to_bf16(k, kb, static_cast<long long>(nb) * Lk * w, st));
-  MSD_TRY(launch_f32_to_bf16(v, vb, static_cast<long long>(nb) * Lk * w, st));
-  if (key_mask) {
-    MSD_TRY(tb.get(&bits, static_cast<size_t>(nb) * (Lk / 32)));
-    MSD_TRY(launch_mask_bits(key_mask, nb, Lk, bits, st));
-  }
-  {
-    AttnArgs aa;
-    memset(&aa, 0, sizeof(aa));
-    aa.Q = qb; aa.ldq = w; aa.K = kb; aa.ldk = w; aa.V = vb; aa.ldv = w; aa.O = ob; aa.ldo = w;
-    aa.nbatch = nb; aa.heads = heads; aa.Lq = Lq; aa.Lk = Lk; aa.mask_bits = bits;
-    aa.mask_stride_words = Lk / 32;
-    float *po = nullptr, *pml = nullptr;
-    MSD_TRY(tb.get(&po, attention_workspace_floats(nb, heads, Lq, 12)));
-    MSD_TRY(tb.get(&pml, static_cast<size_t>(nb) * Lq * heads * 12 * 2));
-    aa.part_o = po; aa.part_ml = pml; aa.max_splits = 12;
-    {
-      const char* f = getenv("MSD_ATTN_SPLITS");  // test hook: force a split count
-      aa.splits = f ? atoi(f) : 0;
-      const char* t = getenv("MSD_ATTN_TAIL");    // test hook: force a tail length
-      aa.tail = t ? atoi(t) : 0;
-    }
-    MSD_TRY(launch_attention(aa, st));
-  }
-  MSD_TRY(launch_bf16_to_f32(ob, out, static_cast<long long>(nb) * Lq * w, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_jax_normal(uint64_t seed, int32_t step, int64_t n, float* out, void* stream) {
-  MSD_REQUIRE(out != nullptr, "msd_op_jax_normal: null argument");
-  uint32_t key[2] = {static_cast<uint32_t>(seed >> 32), static_cast<uint32_t>(seed)};
-  if (step >= 0) {
-    uint32_t folded[2];
-    threefry2x32_host(key[0], key[1], 0u, static_cast<uint32_t>(step), folded);
-    key[0] = folded[0];
-    key[1] = folded[1];
-  }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  MSD_TRY(launch_jax_normal(key[0], key[1], n, out, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_jax_bits(uint64_t seed, int32_t step, int64_t n, uint32_t* out, void* stream) {
-  MSD_REQUIRE(out != nullptr, "msd_op_jax_bits: null argument");
-  uint32_t key[2] = {static_cast<uint32_t>(seed >> 32), static_cast<uint32_t>(seed)};
-  if (step >= 0) {
-    uint32_t folded[2];
-    threefry2x32_host(key[0], key[1], 0u, static_cast<uint32_t>(step), folded);
-    key[0] = folded[0];
-    key[1] = folded[1];
-  }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  MSD_TRY(launch_jax_bits(key[0], key[1], n, out, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_audio_mel(const float* audio, int32_t rows, int64_t n_samples, const float* window,
-                     const float* mel_weights, float* mel_out, void* stream) {
-  MSD_REQUIRE(audio && window && mel_weights && mel_out, "msd_op_audio_mel: null argument");
-  MSD_REQUIRE(rows >= 0 && n_samples >= 0, "msd_op_audio_mel: rows=%d, n_samples=%lld must be >= 0",
-              rows, static_cast<long long>(n_samples));
-  const long long frames = audio_mel_frames(n_samples);
-  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
-              "msd_op_audio_mel: %d rows x %lld frames exceed 2^31 - 1 output frames", rows, frames);
-  MSD_TRY(launch_audio_mel(audio, rows, n_samples, window, mel_weights, mel_out,
-                           reinterpret_cast<cudaStream_t>(stream)));
-  return 0;
-}
-
-int msd_op_audio_resample(const float* x, int32_t rows, int64_t n_in, int32_t orig_sr,
-                          int32_t target_sr, const double* half_window, int32_t window_len,
-                          int32_t precision, const double* time_segments, int32_t n_segments,
-                          float* y, int64_t n_out, void* stream) {
-  MSD_REQUIRE(x && half_window && time_segments && y, "msd_op_audio_resample: null argument");
-  MSD_REQUIRE(rows >= 0 && n_in >= 0 && n_out >= 0,
-              "msd_op_audio_resample: rows=%d, n_in=%lld, n_out=%lld must be >= 0", rows,
-              static_cast<long long>(n_in), static_cast<long long>(n_out));
-  MSD_REQUIRE(orig_sr > 0 && target_sr > 0, "msd_op_audio_resample: rates %d -> %d must be > 0",
-              orig_sr, target_sr);
-  const double ratio = static_cast<double>(target_sr) / orig_sr;
-  const long long want = static_cast<long long>(static_cast<double>(n_in) * ratio);
-  MSD_REQUIRE(n_out == want, "msd_op_audio_resample: n_out=%lld, int(n_in * ratio) is %lld",
-              static_cast<long long>(n_out), want);
-  MSD_REQUIRE(n_in <= INT32_MAX && n_out <= INT32_MAX && rows <= 65535,
-              "msd_op_audio_resample: %d rows x %lld -> %lld samples: at most 65535 rows of "
-              "2^31 - 1 samples", rows, static_cast<long long>(n_in), static_cast<long long>(n_out));
-  MSD_REQUIRE(precision >= 0 && precision <= 24 && window_len >= 2 && n_segments >= 1,
-              "msd_op_audio_resample: precision=%d (0..24), window_len=%d (>= 2), "
-              "n_segments=%d (>= 1)", precision, window_len, n_segments);
-  const int num_table = 1 << precision;
-  MSD_REQUIRE(static_cast<int>((ratio < 1.0 ? ratio : 1.0) * num_table) >= 1,
-              "msd_op_audio_resample: %d -> %d Hz is below one window entry per input sample",
-              orig_sr, target_sr);
-  MSD_TRY(launch_audio_resample(x, rows, static_cast<int>(n_in), ratio, half_window, window_len,
-                                num_table, time_segments, n_segments, y, static_cast<int>(n_out),
-                                reinterpret_cast<cudaStream_t>(stream)));
-  return 0;
-}
-
-int msd_op_griffin_lim_magnitude(const float* features, int32_t rows, int64_t frames,
-                                 const float* mel_weights, const float* pinv, float inv_lipschitz,
-                                 const float* beta, int32_t n_iter, float* mag_out, void* stream) {
-  MSD_REQUIRE(features && mel_weights && pinv && beta && mag_out,
-              "msd_op_griffin_lim_magnitude: null argument");
-  MSD_REQUIRE(rows >= 0 && frames >= 0 && n_iter >= 0,
-              "msd_op_griffin_lim_magnitude: rows=%d, frames=%lld, n_iter=%d must be >= 0", rows,
-              static_cast<long long>(frames), n_iter);
-  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
-              "msd_op_griffin_lim_magnitude: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
-              static_cast<long long>(frames));
-  MSD_TRY(launch_gl_nnls(features, static_cast<long long>(rows) * frames, mel_weights, pinv,
-                         inv_lipschitz, beta, n_iter, mag_out, reinterpret_cast<cudaStream_t>(stream)));
-  return 0;
-}
-
-int msd_op_griffin_lim_init(int32_t rows, int64_t frames, uint64_t seed, float* angles, void* stream) {
-  MSD_REQUIRE(angles, "msd_op_griffin_lim_init: null argument");
-  MSD_REQUIRE(rows >= 0 && frames >= 0, "msd_op_griffin_lim_init: rows=%d, frames=%lld must be >= 0",
-              rows, static_cast<long long>(frames));
-  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
-              "msd_op_griffin_lim_init: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
-              static_cast<long long>(frames));
-  MSD_TRY(launch_gl_phase_init(rows, frames, seed, reinterpret_cast<float2*>(angles),
-                               reinterpret_cast<cudaStream_t>(stream)));
-  return 0;
-}
-
-int msd_op_griffin_lim_iterate(const float* mag, int32_t rows, int64_t frames, const float* window,
-                               float* angles, float* tprev, float* work, float momentum,
-                               int32_t n_iter, void* stream) {
-  MSD_REQUIRE(mag && window && angles && tprev && work, "msd_op_griffin_lim_iterate: null argument");
-  MSD_REQUIRE(rows >= 0 && frames >= 0 && n_iter >= 0,
-              "msd_op_griffin_lim_iterate: rows=%d, frames=%lld, n_iter=%d must be >= 0", rows,
-              static_cast<long long>(frames), n_iter);
-  MSD_REQUIRE(momentum >= 0.f, "msd_op_griffin_lim_iterate: momentum=%g must be >= 0",
-              static_cast<double>(momentum));
-  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
-              "msd_op_griffin_lim_iterate: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
-              static_cast<long long>(frames));
-  MSD_TRY(launch_gl_iterate(mag, rows, frames, window, reinterpret_cast<float2*>(angles),
-                            reinterpret_cast<float2*>(tprev), reinterpret_cast<float2*>(work),
-                            momentum, n_iter, reinterpret_cast<cudaStream_t>(stream)));
-  return 0;
-}
-
-int msd_op_griffin_lim_istft(const float* mag, const float* angles, int32_t rows, int64_t frames,
-                             const float* window, float* audio_out, void* stream) {
-  MSD_REQUIRE(mag && angles && window && audio_out, "msd_op_griffin_lim_istft: null argument");
-  MSD_REQUIRE(rows >= 0 && frames >= 0, "msd_op_griffin_lim_istft: rows=%d, frames=%lld must be >= 0",
-              rows, static_cast<long long>(frames));
-  MSD_REQUIRE(rows == 0 || frames <= INT32_MAX / rows,
-              "msd_op_griffin_lim_istft: %d rows x %lld frames exceed 2^31 - 1 frames", rows,
-              static_cast<long long>(frames));
-  MSD_TRY(launch_gl_istft(mag, reinterpret_cast<const float2*>(angles), rows, frames, window,
-                          audio_out, reinterpret_cast<cudaStream_t>(stream)));
-  return 0;
-}
-
-int msd_op_dense_epilogue(const float* a, const float* w, const float* w1, int32_t M, int32_t N,
-                          int32_t K, int32_t epilogue, int32_t block_n, const float* resid,
-                          const float* pos, int32_t pos_rows, const int32_t* pos_shift,
-                          int32_t dup_rows, float* out, void* stream) {
-  MSD_REQUIRE(a && w && out, "msd_op_dense_epilogue: null argument");
-  const bool gated = epilogue == EPI_GATED_GELU || epilogue == EPI_GATED_GELU_SPLIT3;
-  MSD_REQUIRE(epilogue == EPI_BF16 || epilogue == EPI_RESID_F32 || epilogue == EPI_POS_F32 || gated,
-              "msd_op_dense_epilogue: unknown epilogue %d", epilogue);
-  MSD_REQUIRE(!gated || w1 != nullptr, "msd_op_dense_epilogue: the gated epilogues need w1");
-  MSD_REQUIRE(epilogue != EPI_RESID_F32 || resid != nullptr, "msd_op_dense_epilogue: resid is null");
-  MSD_REQUIRE(epilogue != EPI_POS_F32 || (pos != nullptr && pos_rows > 0),
-              "msd_op_dense_epilogue: pos / pos_rows missing");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const bool split = epilogue == EPI_GATED_GELU_SPLIT3;
-  const int ks = split ? 3 : 1;
-  const int Ng = gated ? 2 * N : N;   // GEMM width
-  TempBufs tb;
-  bf16 *ab = nullptr, *wb = nullptr, *ob = nullptr;
-  MSD_TRY(tb.get(&ab, static_cast<size_t>(M) * K * ks));
-  MSD_TRY(tb.get(&wb, static_cast<size_t>(Ng) * K * ks));
-  if (split) {
-    // A = [hi | lo | hi]: the rmsnorm kernel's split writer with unit gamma would renormalise, so
-    // build it from the scale/split kernel's cousin: plain split of the fp32 values
-    MSD_TRY(launch_split3_rows(a, ab, static_cast<long long>(M), K, st));
-    MSD_TRY(launch_pack_gated(w, w1, K, N, wb, 3 * K, st, 0, 0));
-    MSD_TRY(launch_pack_gated(w, w1, K, N, wb, 3 * K, st, K, 0));
-    MSD_TRY(launch_pack_gated(w, w1, K, N, wb, 3 * K, st, 2 * K, 1));
-  } else {
-    MSD_TRY(launch_f32_to_bf16(a, ab, static_cast<long long>(M) * K, st));
-    if (gated) MSD_TRY(launch_pack_gated(w, w1, K, N, wb, K, st));
-    else MSD_TRY(launch_pack_weight(w, K, N, wb, K, 0, 0, 0, st));
-  }
-  GemmArgs ga;
-  memset(&ga, 0, sizeof(ga));
-  ga.A = ab; ga.B = wb; ga.M = M; ga.N = Ng; ga.K = K * ks; ga.lda = K * ks; ga.ldb = K * ks;
-  ga.epilogue = epilogue; ga.block_n = block_n;
-  ga.resid = resid; ga.pos = pos; ga.pos_rows = pos_rows; ga.pos_shift = pos_shift;
-  ga.dup_rows = dup_rows;
-  const bool bf16_out = epilogue == EPI_BF16 || gated;
-  if (bf16_out) {
-    MSD_TRY(tb.get(&ob, static_cast<size_t>(M) * N * ks));
-    ga.out = ob; ga.ldo = N * ks;
-  } else {
-    ga.out = out; ga.ldo = N;
-  }
-  MSD_TRY(launch_gemm(ga, st));
-  if (bf16_out)
-    MSD_TRY(launch_bf16_rows_to_f32(ob, N * ks, split ? N : 0, out, M, N, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_dense_deferred_norm(const float* a, const float* w_out, const float* x, int32_t M, int32_t d,
-                               int32_t K, const float* g_lo, const float* g_hi, int32_t split_row,
-                               const float* w2, const float* w2b, int32_t N2, const float* bias,
-                               int32_t block_n1, int32_t block_n2, float* x_out, float* y_out,
-                               void* stream) {
-  MSD_REQUIRE(a && w_out && x && g_lo && g_hi && w2 && x_out && y_out,
-              "msd_op_dense_deferred_norm: null argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const bool gated = w2b != nullptr;
-  const int Ng = gated ? 2 * N2 : N2;
-  TempBufs tb;
-  bf16 *ab = nullptr, *wo = nullptr, *opnd = nullptr, *w2p = nullptr, *yb = nullptr;
-  float* ss = nullptr;
-  int* step0 = nullptr;
-  GemmArgs g1;
-  memset(&g1, 0, sizeof(g1));
-  g1.M = M; g1.N = d; g1.K = K; g1.epilogue = EPI_RESID_PREP; g1.block_n = block_n1;
-  const int bn1 = gemm_resolve_block_n(g1);
-  MSD_REQUIRE(bn1 > 0, "msd_op_dense_deferred_norm: no valid tile width for d=%d (block_n1 %d)", d,
-              block_n1);
-  const int parts = d / bn1;
-  MSD_TRY(tb.get(&ab, static_cast<size_t>(M) * K));
-  MSD_TRY(tb.get(&wo, static_cast<size_t>(d) * K));
-  MSD_TRY(tb.get(&opnd, static_cast<size_t>(M) * d));
-  MSD_TRY(tb.get(&w2p, static_cast<size_t>(Ng) * d));
-  MSD_TRY(tb.get(&yb, static_cast<size_t>(M) * N2));
-  MSD_TRY(tb.get(&ss, static_cast<size_t>(parts) * M));
-  MSD_TRY(tb.get(&step0, 1));
-  MSD_CUDA_CHECK(cudaMemsetAsync(step0, 0, sizeof(int), st));
-  MSD_TRY(launch_f32_to_bf16(a, ab, static_cast<long long>(M) * K, st));
-  MSD_TRY(launch_pack_weight(w_out, K, d, wo, K, 0, 0, 0, st));
-  if (gated) MSD_TRY(launch_pack_gated(w2, w2b, d, N2, w2p, d, st));
-  else MSD_TRY(launch_pack_weight(w2, d, N2, w2p, d, 0, 0, 0, st));
-  MSD_CUDA_CHECK(cudaMemcpyAsync(x_out, x, static_cast<size_t>(M) * d * sizeof(float),
-                                 cudaMemcpyDeviceToDevice, st));
-  g1.A = ab; g1.B = wo; g1.lda = K; g1.ldb = K;
-  g1.out = x_out; g1.ldo = d; g1.resid = x_out; g1.block_n = bn1;
-  g1.step = step0;
-  g1.prep.g_lo = g_lo; g1.prep.g_hi = g_hi; g1.prep.split_row = split_row;
-  g1.prep.a = opnd; g1.prep.lda = d; g1.prep.ss = ss; g1.prep.ss_stride = M;
-  MSD_TRY(launch_gemm(g1, st));
-  GemmArgs g2;
-  memset(&g2, 0, sizeof(g2));
-  g2.A = opnd; g2.B = w2p; g2.M = M; g2.N = Ng; g2.K = d; g2.lda = d; g2.ldb = d;
-  g2.epilogue = gated ? EPI_GATED_GELU : EPI_BF16; g2.out = yb; g2.ldo = N2; g2.block_n = block_n2;
-  g2.step = step0;
-  g2.rs.ss_lo = ss; g2.rs.ss_hi = ss; g2.rs.parts_lo = parts; g2.rs.parts_hi = parts;
-  g2.rs.split_row = M; g2.rs.ss_stride = M; g2.rs.inv_d = 1.0f / static_cast<float>(d);
-  g2.rs.col_bias = bias;
-  MSD_TRY(launch_gemm(g2, st));
-  MSD_TRY(launch_bf16_rows_to_f32(yb, N2, 0, y_out, M, N2, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_attention_f32(const float* q, const float* k, const float* v, const int32_t* key_mask,
-                         int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, float* out,
-                         void* stream) {
-  MSD_REQUIRE(q && k && v && out, "msd_op_attention_f32: null argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int w = heads * 64;
-  TempBufs tb;
-  bf16* ob = nullptr;
-  uint32_t* bits = nullptr;
-  MSD_TRY(tb.get(&ob, static_cast<size_t>(nb) * Lq * w * 3));
-  if (key_mask) {
-    MSD_REQUIRE(Lk % 128 == 0, "msd_op_attention_f32: masked Lk must be a multiple of 128");
-    MSD_TRY(tb.get(&bits, static_cast<size_t>(nb) * (Lk / 32)));
-    MSD_TRY(launch_mask_bits(key_mask, nb, Lk, bits, st));
-  }
-  AttnF32Args aa;
-  memset(&aa, 0, sizeof(aa));
-  aa.Q = q; aa.ldq = w; aa.K = k; aa.ldk = w; aa.V = v; aa.ldv = w; aa.O = ob; aa.o_third = w;
-  aa.nbatch = nb; aa.heads = heads; aa.Lq = Lq; aa.Lk = Lk; aa.mask_bits = bits;
-  aa.mask_stride_words = Lk / 32;
-  float *po = nullptr, *pml = nullptr;
-  MSD_TRY(tb.get(&po, static_cast<size_t>(nb) * Lq * heads * 8 * 64));
-  MSD_TRY(tb.get(&pml, static_cast<size_t>(nb) * Lq * heads * 8 * 2));
-  aa.part_o = po; aa.part_ml = pml; aa.max_splits = 8;
-  {
-    const char* f = getenv("MSD_ATTN_SPLITS");  // test hook: force a split count
-    aa.splits = f ? atoi(f) : 0;
-  }
-  MSD_TRY(launch_attention_f32(aa, st));
-  MSD_TRY(launch_bf16_rows_to_f32(ob, 3 * w, w, out, static_cast<long long>(nb) * Lq, w, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq, const void* k,
-                          int64_t k_off, int32_t ldk, const void* v, int64_t v_off, int32_t ldv,
-                          int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32_t kv_batch_rows,
-                          int32_t kv_row0, const int32_t* key_mask, int32_t mask_len,
-                          int32_t mask_word0, int32_t kv_static, void* out, int64_t o_col,
-                          int32_t o_ld, float* part_o, float* part_ml, int32_t splits, int32_t tail,
-                          void* stream) {
-  MSD_REQUIRE(q && k && v && out && part_o && part_ml, "msd_op_attention_view: null argument");
-  MSD_REQUIRE(precision == 0 || precision == 1, "msd_op_attention_view: precision must be 0 or 1");
-  MSD_REQUIRE(nb > 0 && heads > 0 && Lq > 0 && Lk > 0 && q_off >= 0 && k_off >= 0 && v_off >= 0 &&
-                  o_col >= 0 && kv_row0 >= 0 && kv_batch_rows >= 0,
-              "msd_op_attention_view: bad sizes or offsets");
-  MSD_REQUIRE(splits >= 0 && splits <= 12 && tail >= 0 && (precision == 0 || tail == 0),
-              "msd_op_attention_view: splits must be in [0, 12], tail >= 0 (bf16 mode only)");
-  MSD_REQUIRE(!key_mask || (mask_len % 128 == 0 && mask_word0 >= 0 && mask_word0 % 4 == 0 &&
-                            mask_word0 + Lk / 32 <= mask_len / 32),
-              "msd_op_attention_view: mask words [%d, %d) outside rows of %d keys", mask_word0,
-              mask_word0 + Lk / 32, mask_len);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t es = precision ? 4 : 2;
-  const int width = heads * 64;
-  const long long rows_q = static_cast<long long>(nb) * Lq;
-  char* qv = static_cast<char*>(q) + q_off * es;
-  TempBufs tb;
-  uint32_t* bits = nullptr;
-  if (key_mask) {
-    MSD_TRY(tb.get(&bits, static_cast<size_t>(nb) * (mask_len / 32)));
-    MSD_TRY(launch_mask_bits(key_mask, nb, mask_len, bits, st));
-  }
-  // K, V and the mask must be complete before the attention starts (kv_static reads them ahead of
-  // its dependency wait, as after the plain first launch of a diffusion step).  Q is then written
-  // back from a staging copy by a kernel of its own, so that the attention is a PDL launch behind a
-  // live predecessor, as in the step graph.
-  char* stage = nullptr;
-  MSD_TRY(tb.get(&stage, static_cast<size_t>(rows_q) * width * es));
-  MSD_CUDA_CHECK(cudaMemcpy2DAsync(stage, width * es, qv, ldq * es, width * es, rows_q,
-                                   cudaMemcpyDeviceToDevice, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  MSD_TRY(launch_copy_rows(stage, static_cast<long long>(width * es), qv, static_cast<long long>(ldq) * es,
-                           rows_q, static_cast<int>(width * es), st));
-  const uint32_t* mbits = bits ? bits + mask_word0 : nullptr;
-  if (precision == 0) {
-    AttnArgs a;
-    memset(&a, 0, sizeof(a));
-    a.Q = reinterpret_cast<const bf16*>(qv); a.ldq = ldq;
-    a.K = static_cast<const bf16*>(k) + k_off; a.ldk = ldk;
-    a.V = static_cast<const bf16*>(v) + v_off; a.ldv = ldv;
-    a.O = static_cast<bf16*>(out) + o_col; a.ldo = o_ld;
-    a.nbatch = nb; a.heads = heads; a.Lq = Lq; a.Lk = Lk;
-    a.mask_bits = mbits; a.mask_stride_words = mask_len / 32;
-    a.part_o = part_o; a.part_ml = part_ml; a.splits = splits; a.max_splits = 12; a.tail = tail;
-    a.kv_static = kv_static; a.kv_batch_rows = kv_batch_rows; a.kv_row0 = kv_row0;
-    MSD_TRY(launch_attention(a, st));
-  } else {
-    AttnF32Args a;
-    memset(&a, 0, sizeof(a));
-    a.Q = reinterpret_cast<const float*>(qv); a.ldq = ldq;
-    a.K = static_cast<const float*>(k) + k_off; a.ldk = ldk;
-    a.V = static_cast<const float*>(v) + v_off; a.ldv = ldv;
-    a.O = static_cast<bf16*>(out) + o_col; a.o_third = o_ld;
-    a.nbatch = nb; a.heads = heads; a.Lq = Lq; a.Lk = Lk;
-    a.mask_bits = mbits; a.mask_stride_words = mask_len / 32;
-    a.kv_batch_rows = kv_batch_rows; a.kv_row0 = kv_row0;
-    a.part_o = part_o; a.part_ml = part_ml; a.splits = splits; a.max_splits = 12;
-    MSD_TRY(launch_attention_f32(a, st));
-  }
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_gemm_view(const void* a, int64_t a_off, int32_t lda, const void* b, int64_t b_off, int32_t ldb,
-                     int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n, int32_t variant,
-                     void* out, int64_t out_off, int32_t ldo, const float* resid, int64_t resid_off,
-                     const float* pos, int32_t pos_rows, const int32_t* pos_shift, int32_t dup_rows,
-                     const int32_t* step, const float* prep_g_lo, int64_t prep_g_lo_step_stride,
-                     const float* prep_g_hi, int64_t prep_g_hi_step_stride, int32_t prep_split_row,
-                     void* prep_a, int32_t prep_lda, float* prep_ss, int32_t prep_ss_stride,
-                     const float* rs_ss_lo, int32_t rs_parts_lo, const float* rs_ss_hi, int32_t rs_parts_hi,
-                     int32_t rs_split_row, int32_t rs_ss_stride, float rs_inv_d, const float* rs_col_bias,
-                     int64_t rs_bias_step_stride, int32_t* block_n_out, void* stream) {
-  MSD_REQUIRE(a && b && out, "msd_op_gemm_view: null argument");
-  MSD_REQUIRE(epilogue >= EPI_BF16 && epilogue <= EPI_RESID_PREP, "msd_op_gemm_view: unknown epilogue %d",
-              epilogue);
-  MSD_REQUIRE(a_off >= 0 && b_off >= 0 && out_off >= 0 && resid_off >= 0,
-              "msd_op_gemm_view: negative offset");
-  const bool f32_out = epilogue == EPI_F32 || epilogue == EPI_RESID_F32 || epilogue == EPI_POS_F32 ||
-                       epilogue == EPI_RESID_PREP;
-  GemmArgs g;
-  memset(&g, 0, sizeof(g));
-  g.A = static_cast<const bf16*>(a) + a_off; g.lda = lda;
-  g.B = static_cast<const bf16*>(b) + b_off; g.ldb = ldb;
-  g.M = M; g.N = N; g.K = K; g.epilogue = epilogue; g.block_n = block_n; g.variant = variant;
-  g.out = f32_out ? static_cast<void*>(static_cast<float*>(out) + out_off)
-                  : static_cast<void*>(static_cast<bf16*>(out) + out_off);
-  g.ldo = ldo;
-  g.resid = resid ? resid + resid_off : nullptr;
-  g.pos = pos; g.pos_rows = pos_rows; g.pos_shift = pos_shift; g.dup_rows = dup_rows;
-  g.step = step;
-  g.prep.g_lo = prep_g_lo; g.prep.g_lo_step_stride = prep_g_lo_step_stride;
-  g.prep.g_hi = prep_g_hi; g.prep.g_hi_step_stride = prep_g_hi_step_stride;
-  g.prep.split_row = prep_split_row;
-  g.prep.a = static_cast<bf16*>(prep_a); g.prep.lda = prep_lda;
-  g.prep.ss = prep_ss; g.prep.ss_stride = prep_ss_stride;
-  g.rs.ss_lo = rs_ss_lo; g.rs.parts_lo = rs_parts_lo; g.rs.ss_hi = rs_ss_hi; g.rs.parts_hi = rs_parts_hi;
-  g.rs.split_row = rs_split_row; g.rs.ss_stride = rs_ss_stride; g.rs.inv_d = rs_inv_d;
-  g.rs.col_bias = rs_col_bias; g.rs.bias_step_stride = rs_bias_step_stride;
-  MSD_REQUIRE(epilogue != EPI_RESID_PREP || g.prep.a != nullptr,
-              "msd_op_gemm_view: EPI_RESID_PREP needs prep_a");
-  MSD_REQUIRE(epilogue != EPI_POS_F32 || (pos != nullptr && pos_rows > 0),
-              "msd_op_gemm_view: EPI_POS_F32 needs pos / pos_rows");
-  const int bn = gemm_resolve_block_n(g);
-  MSD_REQUIRE(bn > 0, "msd_op_gemm_view: N=%d has no tile width (block_n %d, variant %d)", N, block_n, variant);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  g_pdl_skip_next = true;   // the operands were just written by the caller's own kernels
-  MSD_TRY(launch_gemm(g, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  if (block_n_out) *block_n_out = bn;
-  return 0;
-}
-
-int msd_op_prep_rows(const float* x, const float* g, int64_t g_step_stride, const int32_t* step, int32_t rows,
-                     int32_t d, void* a_out, int32_t lda, float* ss_out, void* stream) {
-  MSD_REQUIRE(x && g && step && a_out && ss_out, "msd_op_prep_rows: null argument");
-  MSD_REQUIRE(rows > 0 && lda >= d && lda % 8 == 0, "msd_op_prep_rows: rows %d / lda %d (d %d)", rows, lda, d);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  g_pdl_skip_next = true;
-  MSD_TRY(launch_prep_rows(x, g, g_step_stride, step, rows, d, static_cast<bf16*>(a_out), lda, ss_out, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_sampler_step(const float* eps, float* z, void* z_split, float* mel_out, const float* noise,
-                        const float* coef, int32_t num_steps, const int32_t* step, int64_t n, int32_t n_dims,
-                        int32_t passes, float cond_weight, int32_t clip_x0, int32_t ddim, float feat_min,
-                        float feat_max, uint64_t seed, int32_t rng_kind, const uint32_t* rng_keys,
-                        int64_t n_row, const uint32_t* row_keys, int64_t row_key_stride,
-                        const uint64_t* row_seeds, int32_t run_step, int32_t per_row, int32_t launches,
-                        int32_t* run_out, void* stream) {
-  MSD_REQUIRE(eps && z && z_split && coef, "msd_op_sampler_step: null argument");
-  MSD_REQUIRE(n > 0 && n_dims > 0 && n % 4 == 0 && n_dims % 4 == 0 && n % n_dims == 0 && num_steps > 0,
-              "msd_op_sampler_step: n=%lld must be a positive multiple of n_dims=%d, both multiples of 4",
-              static_cast<long long>(n), n_dims);
-  MSD_REQUIRE(passes == 1 || passes == 2, "msd_op_sampler_step: passes must be 1 or 2 (got %d)", passes);
-  MSD_REQUIRE(rng_kind == 0 || rng_kind == 1, "msd_op_sampler_step: rng_kind must be 0 or 1");
-  MSD_REQUIRE(rng_kind == 0 || per_row || (rng_keys != nullptr && n % 8 == 0 && n < (1ll << 32)),
-              "msd_op_sampler_step: the jax stream needs its key table and a draw of k*8 < 2^32 elements");
-  MSD_REQUIRE(!per_row || (n_row > 0 && n_row % 8 == 0 && n % n_row == 0 && n < (1ll << 32) &&
-                           (rng_kind == 0 ? row_seeds != nullptr : row_keys != nullptr)),
-              "msd_op_sampler_step: per-row streams need rows of k*8 elements, n < 2^32 and the row table");
-  MSD_REQUIRE(step == nullptr || (!per_row && launches == 1),
-              "msd_op_sampler_step: per-row streams and several launches need the RunArgs path (step NULL)");
-  MSD_REQUIRE(step != nullptr || run_out != nullptr, "msd_op_sampler_step: the RunArgs path needs run_out");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int first = run_step;
-  if (step != nullptr) MSD_CUDA_CHECK(cudaMemcpy(&first, step, sizeof(int), cudaMemcpyDeviceToHost));
-  MSD_REQUIRE(launches >= 1 && first < num_steps && first - launches + 1 >= 0,
-              "msd_op_sampler_step: %d launch(es) from step %d leave the table of %d steps", launches, first,
-              num_steps);
-  SamplerArgs a;
-  memset(&a, 0, sizeof(a));
-  a.eps = eps; a.z = z; a.z_split = static_cast<bf16*>(z_split); a.coef = coef;
-  a.n = n; a.n_dims = n_dims; a.passes = passes; a.cond_weight = cond_weight;
-  a.clip_x0 = clip_x0; a.ddim = ddim; a.feat_min = feat_min; a.feat_max = feat_max;
-  a.rng_kind = rng_kind; a.rng_keys = rng_keys;
-  a.n_row = n_row; a.row_keys = row_keys; a.row_key_stride = row_key_stride;
-  a.row_seeds = reinterpret_cast<const unsigned long long*>(row_seeds);
-  TempBufs tb;
-  if (step != nullptr) {
-    a.step = step; a.noise = noise; a.mel_out = mel_out; a.seed = seed;
-    g_pdl_skip_next = true;   // the inputs were just written by the caller's own kernels
-    MSD_TRY(launch_sampler_step(a, st));
-    MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-    return 0;
-  }
-  RunArgs ra;
-  memset(&ra, 0, sizeof(ra));
-  ra.noise = noise; ra.mel_out = mel_out; ra.seed = seed; ra.step = run_step; ra.per_row = per_row;
-  MSD_TRY(tb.get(&a.run, 1));
-  MSD_CUDA_CHECK(cudaMemcpyAsync(a.run, &ra, sizeof(ra), cudaMemcpyHostToDevice, st));
-  // the first launch follows the upload; the next ones are PDL launches behind the previous step's
-  // sampler kernel, which is what the step graph's first kernel sees
-  g_pdl_skip_next = true;
-  for (int i = 0; i < launches; ++i) MSD_TRY(launch_sampler_step(a, st));
-  MSD_CUDA_CHECK(cudaMemcpyAsync(&ra, a.run, sizeof(ra), cudaMemcpyDeviceToHost, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  run_out[0] = ra.step;
-  run_out[1] = static_cast<int32_t>(ra.done);
-  return 0;
-}
-
-int msd_op_init_z(const float* init_z, float* z, void* z_split, int64_t n, int32_t n_dims, uint64_t seed,
-                  int32_t rng_kind, const uint32_t* rng_keys, int64_t n_row, int64_t row_key_stride,
-                  const uint64_t* row_seeds, void* stream) {
-  MSD_REQUIRE(z && z_split, "msd_op_init_z: null argument");
-  MSD_REQUIRE(n > 0 && n_dims > 0 && n % 4 == 0 && n_dims % 4 == 0 && n % n_dims == 0,
-              "msd_op_init_z: n=%lld must be a positive multiple of n_dims=%d, both multiples of 4",
-              static_cast<long long>(n), n_dims);
-  MSD_REQUIRE(rng_kind == 0 || rng_kind == 1, "msd_op_init_z: rng_kind must be 0 or 1");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  MSD_TRY(launch_init_z(init_z, z, static_cast<bf16*>(z_split), n, n_dims, seed, st, rng_kind, rng_keys, n_row,
-                        row_key_stride, reinterpret_cast<const unsigned long long*>(row_seeds)));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
-int msd_op_scale_split(const float* feat, void* out_split, int64_t rows, int32_t n_dims, float feat_min,
-                       float feat_max, void* stream) {
-  MSD_REQUIRE(feat && out_split, "msd_op_scale_split: null argument");
-  MSD_REQUIRE(rows > 0 && n_dims > 0 && n_dims % 4 == 0, "msd_op_scale_split: rows %lld / n_dims %d",
-              static_cast<long long>(rows), n_dims);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  MSD_TRY(launch_scale_split(feat, static_cast<bf16*>(out_split), rows, n_dims, feat_min, feat_max, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
 int msd_get_conditioning_tables(msd_ctx* c, float* film, float* gain, float* bias_qkv, float* bias_wi) {
   MSD_REQUIRE(c != nullptr, "msd_get_conditioning_tables: null context");
   MSD_REQUIRE(c->weights_loaded, "msd_get_conditioning_tables: call msd_load_weights first");
@@ -2295,21 +1485,4 @@ int msd_get_conditioning_tables(msd_ctx* c, float* film, float* gain, float* bia
     if (t.dst) MSD_CUDA_CHECK(cudaMemcpy(t.dst, t.src, t.n * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
-
-int msd_op_rmsnorm_film(const float* x, const float* gamma, const float* film, int32_t rows,
-                        int32_t d, float* out, void* stream) {
-  MSD_REQUIRE(x && gamma && out, "msd_op_rmsnorm_film: null argument");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  TempBufs tb;
-  bf16* ob = nullptr;
-  int* zero = nullptr;
-  MSD_TRY(tb.get(&ob, static_cast<size_t>(rows) * d));
-  MSD_TRY(tb.get(&zero, 1));
-  MSD_CUDA_CHECK(cudaMemsetAsync(zero, 0, sizeof(int), st));
-  MSD_TRY(launch_rmsnorm(x, gamma, rows, d, ob, d, film, zero, 0, 0, 0, st));
-  MSD_TRY(launch_bf16_to_f32(ob, out, static_cast<long long>(rows) * d, st));
-  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  return 0;
-}
-
 }  // extern "C"
