@@ -41,7 +41,10 @@ typedef struct msd_config {
   int32_t mlp_dim;               /* gated ('gelu','linear') MLP; multiple of 64 */
   int32_t inputs_length;         /* token positions, multiple of 128 */
   int32_t targets_length;        /* mel frames per segment, multiple of 128 */
-  int32_t context_length;        /* context frames, multiple of 128 */
+  int32_t context_length;        /* context frames, multiple of 128; 0 selects the no-context model
+                                    (models.DiffusionModel + network.Transformer, network.py:
+                                    460-496): token encoder `encoder/...`, no continuous encoder,
+                                    one cross-attention source for either cross_attend_style */
   int32_t n_dims;                /* mel bins, must be 128 */
   int32_t num_steps;             /* sampler schedule num_steps */
   int32_t max_batch;             /* segments per call (B) */
@@ -104,7 +107,10 @@ int msd_load_weights(msd_ctx* ctx, const msd_tensor* tensors, int32_t n);
  * (models/diffusion/models.py:361-371; network.py:537-559) and additionally projects the
  * concatenated encodings to every decoder layer's cross-attention K/V once (network.py:217-230
  * is loop-invariant).  tokens [B, inputs_length] int32, ctx_features [B, context_length,
- * n_dims] f32 in codec feature units, ctx_mask [B, context_length] int32: device pointers. */
+ * n_dims] f32 in codec feature units, ctx_mask [B, context_length] int32: device pointers.
+ * With context_length == 0 (DiffusionModel.predict_batch_with_aux + Transformer.encode,
+ * models.py:149-205, network.py:470-482) only the tokens are encoded; ctx_features and ctx_mask
+ * are not read and may be NULL. */
 int msd_encode(msd_ctx* ctx, const int32_t* tokens, const float* ctx_features,
                const int32_t* ctx_mask, int32_t batch, void* stream);
 
@@ -149,7 +155,8 @@ int msd_decode_eps(msd_ctx* ctx, const float* z, int32_t step_i, int32_t conditi
                    float* eps_out, void* stream);
 
 /* Test hook: copies the encoder outputs of the last msd_encode as bf16-rounded f32:
- * enc_out [B, inputs_length + context_length, emb_dim] device f32. */
+ * enc_out [B, inputs_length + context_length, emb_dim] device f32 ([B, inputs_length, emb_dim]
+ * with context_length == 0). */
 int msd_get_encodings(msd_ctx* ctx, float* enc_out, void* stream);
 
 /* Host copy of the per-step sampler scalars [num_steps][16]:

@@ -6,6 +6,8 @@
 // Reference call stack replaced (SURVEY §3.1):
 //   ContextDiffusionModel.predict_batch_with_aux   msd/models/diffusion/models.py:340-400
 //   ContinuousContextTransformer.encode / .decode  msd/models/diffusion/network.py:537-573
+//   (context_length == 0: DiffusionModel.predict_batch_with_aux, models.py:149-205, and
+//    Transformer.encode / .decode, network.py:470-496: the same decoder, no context encoder)
 //   eval_scan / eval_step / ddpm_step              msd/models/diffusion/diffusion_utils.py:382-476
 //
 // Exact algebraic shortcuts relative to the graph as written (each proven equal to the oracle
@@ -185,6 +187,9 @@ struct msd_ctx {
   int device = 0;
   // derived sizes
   int d = 0, H = 0, hh = 0, F = 0, T = 0, N = 0, C = 0, Mkv = 0, nd = 0, Bmax = 0, passes = 2;
+  // cross-attention sources attended one by one: 2 for sum_cross_attends with a context, else 1
+  // (one source, or the concatenated [tokens | context] of concat_encodings)
+  int nsrc = 1;
   // fp32-accurate mode (cfg.precision == 1): every GEMM runs as a 3 x bf16 split-precision product
   // (A = [hi | lo | hi], W = [hi | hi | lo], K tripled: ks == 3), q/k/v and the cross K/V cache
   // are fp32, attention is the fp32 kernel and its output / the gated-GELU output are split again.
@@ -199,7 +204,7 @@ struct msd_ctx {
   // ---- parameters
   float* tok_emb = nullptr;  // [vocab, d] f32
   Encoder tok_enc, ctx_enc;
-  bf16* ctx_in_proj = nullptr;  // [d, 3*nd] split [hi|hi|lo]
+  bf16* ctx_in_proj = nullptr;  // [d, 3*nd] split [hi|hi|lo]; none without a context
   bf16* dec_in_proj = nullptr;  // [d, 3*nd]
   float* dec_pos = nullptr;     // [N, d]
   std::vector<DecLayer> dec;
@@ -250,7 +255,7 @@ struct msd_ctx {
   bf16* eqkv = nullptr;
   bf16* eattn = nullptr;
   bf16* eh = nullptr;
-  bf16* ctx_split = nullptr;  // [B*C, 3*nd]
+  bf16* ctx_split = nullptr;  // [B*C, 3*nd]; none without a context
   uint32_t* mask_bits = nullptr;  // [B, Mkv/32]
   int* ctx_seq_len = nullptr;     // [B]
   RunArgs* run = nullptr;         // per-call arguments + step index, device memory
@@ -597,12 +602,17 @@ static int load_all(msd_ctx* c, Loader& L) {
   Arena& A = c->arena;
   const msd_config& g = c->cfg;
   const int d = c->d, hh = c->hh, F = c->F, nd = c->nd;
-  MSD_TRY(load_f32(L, A, "token_encoder/token_embedder/embedding", g.vocab_size, d, &c->tok_emb));
-  MSD_TRY(load_encoder(L, A, "token_encoder", g.num_encoder_layers, c->T, d, hh, F, &c->tok_enc));
-  MSD_TRY(load_encoder(L, A, "continuous_encoder", g.num_encoder_layers, c->C, d, hh, F,
-                       &c->ctx_enc));
-  MSD_TRY(A.alloc(&c->ctx_in_proj, static_cast<size_t>(d) * 3 * nd));
-  MSD_TRY(pack_split3(L, "continuous_encoder/input_proj/kernel", nd, d, c->ctx_in_proj));
+  // ContinuousContextTransformer names its token encoder `token_encoder` (network.py:530-535),
+  // Transformer `encoder` (network.py:467), and has no continuous encoder
+  const std::string tok = c->C > 0 ? "token_encoder" : "encoder";
+  MSD_TRY(load_f32(L, A, tok + "/token_embedder/embedding", g.vocab_size, d, &c->tok_emb));
+  MSD_TRY(load_encoder(L, A, tok, g.num_encoder_layers, c->T, d, hh, F, &c->tok_enc));
+  if (c->C > 0) {
+    MSD_TRY(load_encoder(L, A, "continuous_encoder", g.num_encoder_layers, c->C, d, hh, F,
+                         &c->ctx_enc));
+    MSD_TRY(A.alloc(&c->ctx_in_proj, static_cast<size_t>(d) * 3 * nd));
+    MSD_TRY(pack_split3(L, "continuous_encoder/input_proj/kernel", nd, d, c->ctx_in_proj));
+  }
   MSD_TRY(A.alloc(&c->dec_in_proj, static_cast<size_t>(d) * 3 * nd));
   MSD_TRY(pack_split3(L, "decoder/continuous_inputs_projection/kernel", nd, d, c->dec_in_proj));
   MSD_TRY(load_f32(L, A, "decoder/Embed_0/embedding", c->N, d, &c->dec_pos));
@@ -613,7 +623,7 @@ static int load_all(msd_ctx* c, Loader& L) {
     MSD_TRY(load_f32(L, A, p + "/pre_self_attention_layer_norm/scale", d, 1, &dl.ln_self));
     MSD_TRY(load_attn(L, A, p + "/self_attention", d, hh, &dl.self_attn));
     MSD_TRY(load_f32(L, A, p + "/pre_cross_attention_layer_norm/scale", d, 1, &dl.ln_cross));
-    const int nsrc = g.cross_attend_style == 1 ? 2 : 1;
+    const int nsrc = c->nsrc;
     MSD_TRY(A.alloc(&dl.cross_q, static_cast<size_t>(nsrc) * hh * d * L.ks));
     MSD_TRY(A.alloc(&dl.cross_kv, static_cast<size_t>(2) * hh * d * L.ks));
     if (nsrc == 2) MSD_TRY(A.alloc(&dl.cross_kv1, static_cast<size_t>(2) * hh * d * L.ks));
@@ -736,14 +746,15 @@ static int run_encoder(msd_ctx* c, const Encoder& e, int B, int len, const uint3
 // (network.py:196-235), into `o`, the input buffer of the output projection.  concat_encodings
 // attends the concatenated [tokens | context] cache once; sum_cross_attends runs one attention
 // per source (each zeroed where its source is fully masked) into the two halves of `o`, which the
-// stacked output projection sums.
+// stacked output projection sums.  With one source (no context) the two styles are the same
+// computation (network.py:199-235) and both attend the T token keys once.
 static int cross_attention(const msd_ctx* c, int l, int nseg, bf16* o, cudaStream_t st) {
   const int hh = c->hh, N = c->N, words = c->Mkv / 32;
   const size_t kv = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;  // elements
   AttnView ex = {};
   ex.part_o = c->attn_part_o; ex.part_ml = c->attn_part_ml;
   ex.kv_static = 1;
-  if (c->cfg.cross_attend_style == 0)
+  if (c->nsrc == 1)
     return attention(c, c->qc, 0, hh, c->kv_cache, kv, 2 * hh, c->kv_cache, kv + hh, 2 * hh, o, hh, 0, nseg,
                      c->H, N, c->Mkv, c->mask_bits, words, st, ex);
   ex.kv_batch_rows = c->Mkv;
@@ -865,7 +876,7 @@ static int decoder_layers(msd_ctx* c, int seg0, int nseg, int ncross, cudaStream
   const int d = c->d, hh = c->hh, F = c->F, N = c->N, ks = c->ks;
   const int R = nseg * N, Rc = ncross * N;
   const int Ld = c->cfg.num_decoder_layers;
-  const int nsrc = c->cfg.cross_attend_style == 1 ? 2 : 1;
+  const int nsrc = c->nsrc;
   const size_t r0 = static_cast<size_t>(seg0) * N;
   // views of the row buffers (disjoint per range); a GEMM-input row is ks x wider
   const LayerRows s = {c, Rc, c->x + r0 * d, c->xn + r0 * d * ks, st};
@@ -988,6 +999,7 @@ static int validate(const msd_config* g) {
   MSD_REQUIRE(g->inputs_length % 128 == 0 && g->targets_length % 128 == 0 &&
                   g->context_length % 128 == 0,
               "sequence lengths must be multiples of 128");
+  MSD_REQUIRE(g->context_length >= 0, "context_length must be >= 0 (0: no context, network.Transformer)");
   MSD_REQUIRE(g->num_steps > 0 && g->max_batch > 0, "num_steps and max_batch must be positive");
   MSD_REQUIRE(g->sampler == 0 || g->sampler == 1, "sampler must be 0 (ddpm) or 1 (ddim)");
   MSD_REQUIRE(g->logvar_type >= 0 && g->logvar_type <= 2, "logvar_type must be 0, 1 or 2");
@@ -1047,6 +1059,7 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   c->d = cfg->emb_dim; c->H = cfg->num_heads; c->hh = cfg->num_heads * 64; c->F = cfg->mlp_dim;
   c->T = cfg->inputs_length; c->N = cfg->targets_length; c->C = cfg->context_length;
   c->Mkv = c->T + c->C; c->nd = cfg->n_dims; c->Bmax = cfg->max_batch;
+  c->nsrc = (cfg->cross_attend_style == 1 && c->C > 0) ? 2 : 1;
   c->passes = (cfg->eval_condition_weight != 1.0f) ? 2 : 1;
   c->acc = cfg->precision == 1;
   c->ks = c->acc ? 3 : 1;
@@ -1074,13 +1087,13 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   MSD_TRY(A.alloc(&c->qkv, R * 3 * c->hh * qe));
   MSD_TRY(A.alloc(&c->attn, R * c->hh * ks));
   MSD_TRY(A.alloc(&c->hmid, R * c->F * ks));
-  MSD_TRY(A.alloc(&c->qc, BN * c->hh * (cfg->cross_attend_style == 1 ? 2 : 1) * qe));
-  if (cfg->cross_attend_style == 1) MSD_TRY(A.alloc(&c->attn2, BN * 2 * c->hh * ks));
+  MSD_TRY(A.alloc(&c->qc, BN * c->hh * c->nsrc * qe));
+  if (c->nsrc == 2) MSD_TRY(A.alloc(&c->attn2, BN * 2 * c->hh * ks));
   const size_t npart = attention_workspace_floats(c->Bmax, c->H, c->N, kMaxSplits);
   MSD_TRY(A.alloc(&c->attn_part_o, npart));
   MSD_TRY(A.alloc(&c->attn_part_ml, BN * c->H * kMaxSplits * 2));
   c->attn_part_o2 = c->attn_part_o; c->attn_part_ml2 = c->attn_part_ml;
-  if (cfg->cross_attend_style == 1) {
+  if (c->nsrc == 2) {
     MSD_TRY(A.alloc(&c->attn_part_o2, npart));
     MSD_TRY(A.alloc(&c->attn_part_ml2, BN * c->H * kMaxSplits * 2));
   }
@@ -1105,7 +1118,7 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   MSD_TRY(A.alloc(&c->eqkv, ER * 3 * c->hh * qe));
   MSD_TRY(A.alloc(&c->eattn, ER * c->hh * ks));
   MSD_TRY(A.alloc(&c->eh, ER * c->F * ks));
-  MSD_TRY(A.alloc(&c->ctx_split, static_cast<size_t>(c->Bmax) * c->C * 3 * c->nd));
+  if (c->C > 0) MSD_TRY(A.alloc(&c->ctx_split, static_cast<size_t>(c->Bmax) * c->C * 3 * c->nd));
   MSD_TRY(A.alloc(&c->mask_bits, static_cast<size_t>(c->Bmax) * (c->Mkv / 32)));
   MSD_TRY(A.alloc(&c->ctx_seq_len, static_cast<size_t>(c->Bmax)));
   MSD_TRY(A.alloc(&c->run, 1));
@@ -1187,30 +1200,34 @@ static int end_on(msd_ctx* c, cudaStream_t caller) {
 
 int msd_encode(msd_ctx* c, const int32_t* tokens, const float* ctx_features,
                const int32_t* ctx_mask, int32_t batch, void* stream) {
-  MSD_REQUIRE(c && tokens && ctx_features && ctx_mask, "msd_encode: null argument");
+  MSD_REQUIRE(c && tokens, "msd_encode: null argument");
+  MSD_REQUIRE(c->C == 0 || (ctx_features && ctx_mask), "msd_encode: null context argument");
   MSD_REQUIRE(c->weights_loaded, "msd_encode: call msd_load_weights first");
   MSD_REQUIRE(batch >= 1 && batch <= c->Bmax, "msd_encode: batch %d outside [1, %d]", batch, c->Bmax);
   cudaStream_t caller = reinterpret_cast<cudaStream_t>(stream);
   MSD_TRY(begin_on(c, caller));
   cudaStream_t st = c->work;
   const int B = batch, d = c->d, hh = c->hh, nd = c->nd;
+  // without a context the mask rows hold the token words only, and there is no roll to compute
   MSD_TRY(launch_build_masks(tokens, ctx_mask, B, c->T, c->C, c->mask_bits, c->ctx_seq_len,
-                             c->cfg.context_positions, st));
+                             c->C > 0 ? c->cfg.context_positions : 0, st));
   // token encoder (network.py:261-303)
   MSD_TRY(launch_embed_tokens(tokens, c->tok_emb, c->tok_enc.pos, c->ex, B, c->T, d,
                               c->cfg.vocab_size, st));
   MSD_TRY(run_encoder(c, c->tok_enc, B, c->T, c->mask_bits, 0, st));
-  // continuous encoder (models.py:361-363 scale_features; network.py:306-357)
-  MSD_TRY(launch_scale_split(ctx_features, c->ctx_split, static_cast<long long>(B) * c->C, nd,
-                             c->cfg.feature_min, c->cfg.feature_max, st));
-  MSD_TRY(gemm_pos(c->ctx_split, 3 * nd, c->ctx_in_proj, 3 * nd, B * c->C, d, 3 * nd, c->ex,
-                   c->ctx_enc.pos, c->C, c->ctx_seq_len, 0, st));
-  MSD_TRY(run_encoder(c, c->ctx_enc, B, c->C, c->mask_bits + c->T / 32, c->T, st));
+  if (c->C > 0) {
+    // continuous encoder (models.py:361-363 scale_features; network.py:306-357)
+    MSD_TRY(launch_scale_split(ctx_features, c->ctx_split, static_cast<long long>(B) * c->C, nd,
+                               c->cfg.feature_min, c->cfg.feature_max, st));
+    MSD_TRY(gemm_pos(c->ctx_split, 3 * nd, c->ctx_in_proj, 3 * nd, B * c->C, d, 3 * nd, c->ex,
+                     c->ctx_enc.pos, c->C, c->ctx_seq_len, 0, st));
+    MSD_TRY(run_encoder(c, c->ctx_enc, B, c->C, c->mask_bits + c->T / 32, c->T, st));
+  }
   // cross-attention K/V of every decoder layer, once per segment batch
   const size_t dk = static_cast<size_t>(d) * c->ks;  // row length of the encodings buffer
   for (int l = 0; l < c->cfg.num_decoder_layers; ++l) {
     const size_t kv_off = static_cast<size_t>(l) * c->Bmax * c->Mkv * 2 * hh;  // elements
-    if (c->cfg.cross_attend_style == 0) {
+    if (c->nsrc == 1) {
       MSD_TRY(dense(c, c->enc, c->dec[l].cross_kv, B * c->Mkv, 2 * hh, d, epi_qkv(c),
                     at(c, c->kv_cache, kv_off), 2 * hh, nullptr, st));
       continue;

@@ -31,7 +31,10 @@ def make_msd_config(t5: T5Config, diffusion: DiffusionConfig, inputs_length: int
   """Translate the reference's config objects into `struct msd_config`.  rng: 'jax' (the
   threefry stream of jax.random.PRNGKey(seed), as the reference draws its noise) or 'philox'.
   precision: 'bf16' (tensor-core operands in bf16, the fast path) or 'fp32_accurate' (3 x bf16
-  split-precision dense layers + fp32 attention: what T5Config.dtype = float32 asks for)."""
+  split-precision dense layers + fp32 attention: what T5Config.dtype = float32 asks for).
+  context_length 0 (or None) selects the no-context model, models.DiffusionModel with
+  network.Transformer (gin/models/diffusion/basic)."""
+  context_length = int(context_length or 0)
   if rng not in ('jax', 'philox'):
     raise ValueError(f'unknown rng {rng!r}')
   if precision not in PRECISIONS:
@@ -142,15 +145,25 @@ class Engine:
     _native.check(self.lib.msd_load_weights(self._h, arr, len(names)), 'msd_load_weights')
 
   # -- operator surface --------------------------------------------------------
-  def encode(self, tokens: torch.Tensor, ctx_features: torch.Tensor,
-             ctx_mask: torch.Tensor) -> None:
+  def encode(self, tokens: torch.Tensor, ctx_features: Optional[torch.Tensor],
+             ctx_mask: Optional[torch.Tensor]) -> None:
+    """ctx_features / ctx_mask: the context, or None for both with a no-context model
+    (context_length 0)."""
     b = tokens.shape[0]
     assert tokens.dtype == torch.int32 and tokens.is_cuda and tokens.is_contiguous()
-    assert ctx_features.dtype == torch.float32 and ctx_features.is_contiguous()
-    assert ctx_mask.dtype == torch.int32 and ctx_mask.is_contiguous()
     assert tokens.shape == (b, self.cfg.inputs_length), tokens.shape
-    assert ctx_features.shape == (b, self.cfg.context_length, self.cfg.n_dims)
-    assert ctx_mask.shape == (b, self.cfg.context_length)
+    if self.cfg.context_length == 0:
+      if ctx_features is not None or ctx_mask is not None:
+        raise ValueError('this model has no context (context_length 0): pass None for '
+                         'ctx_features and ctx_mask')
+    else:
+      if ctx_features is None or ctx_mask is None:
+        raise ValueError(f'this model takes a context of {self.cfg.context_length} frames: '
+                         'ctx_features and ctx_mask are required')
+      assert ctx_features.dtype == torch.float32 and ctx_features.is_contiguous()
+      assert ctx_mask.dtype == torch.int32 and ctx_mask.is_contiguous()
+      assert ctx_features.shape == (b, self.cfg.context_length, self.cfg.n_dims)
+      assert ctx_mask.shape == (b, self.cfg.context_length)
     _native.check(self.lib.msd_encode(self._h, _ptr(tokens), _ptr(ctx_features), _ptr(ctx_mask),
                                       b, _stream(self.device)), 'msd_encode')
     self._batch = b

@@ -10,6 +10,12 @@ Keeps the reference's call surface:
 and replaces the jitted `predict_batch_with_aux` with libmsd_b200.so (ctypes; torch only
 allocates device/pinned buffers).  There is no CPU fallback.
 
+Both diffusion model families of the reference run: `models.ContextDiffusionModel` +
+`network.ContinuousContextTransformer` (TASK_FEATURE_LENGTHS with `targets_context`, the
+gin/models/diffusion/context configs) and the no-context `models.DiffusionModel` +
+`network.Transformer` (lengths without `targets_context`, gin/models/diffusion/basic).  As in the
+reference, the lengths decide which inputs the model takes (inference.py:113-157).
+
 Checkpoints: `checkpoint_path` may be a T5X checkpoint directory such as
 `.../base_with_context/checkpoint_500000` (msgpack index + one zarr array per parameter, read by
 `t5x_checkpoint.py` without t5x/tensorstore), an `.npz` written by `weights.save_npz` (flax
@@ -51,6 +57,18 @@ def parse_training_gin_file(gin_file: str, gin_bindings: Sequence[str]) -> str:
 
 
 # ---- minimal stand-ins for objects callers poke at --------------------------------------
+class _NoContextFeatureConverterSpec:
+  """Batch-dict schema of ContinuousOutpusEncDecFeatureConverter (msd/feature_converters.py:23-39),
+  the feature converter of the no-context DiffusionModel (models.py:38)."""
+  TASK_FEATURES = {'inputs': np.int32, 'targets': np.float32}
+  MODEL_FEATURES = {
+      'encoder_input_tokens': np.int32,
+      'decoder_target_tokens': np.float32,
+      'decoder_input_tokens': np.float32,
+      'decoder_target_mask': np.bool_,
+  }
+
+
 class _FeatureConverterSpec:
   """Batch-dict schema of ContinuousContextFeatureConverter
   (msd/models/diffusion/feature_converters.py:26-43)."""
@@ -96,10 +114,32 @@ def num_embeddings(codec: midi_tokens.EventVocabulary, extra_ids: int = 100) -> 
   return 128 * math.ceil(vocab_size / 128)
 
 
+# MODEL macro -> whether the model takes a context (TASK_FEATURE_LENGTHS has `targets_context`)
+_DIFFUSION_MODELS = {'DiffusionModel': False, 'ContextDiffusionModel': True}
+
+
+def _check_model_lengths(model: Any, lengths: Mapping[str, int]) -> None:
+  """models.DiffusionModel runs without a context and models.ContextDiffusionModel with one; the
+  task's lengths must say the same (the reference fails later, inside its feature converter)."""
+  if not isinstance(model, gin_lite.ConfigurableRef):
+    return
+  name = model.name.rsplit('.', 1)[-1]
+  if name not in _DIFFUSION_MODELS:
+    return
+  with_context = 'targets_context' in lengths
+  if _DIFFUSION_MODELS[name] != with_context:
+    raise ValueError(
+        f'MODEL = @{model.name}() needs TASK_FEATURE_LENGTHS '
+        f'{"with" if _DIFFUSION_MODELS[name] else "without"} targets_context, got {dict(lengths)}: '
+        'models.ContextDiffusionModel takes inputs, targets and targets_context, '
+        'models.DiffusionModel inputs and targets only')
+
+
 def _build_from_gin(gin_config: str) -> Tuple[config.T5Config, config.DiffusionConfig,
                                               Dict[str, int], midi_tokens.EventVocabulary]:
   g = gin_lite.parse_config(gin_config, _GIN_SEARCH_ROOTS)
   lengths = dict(g.query_macro('TASK_FEATURE_LENGTHS'))
+  _check_model_lengths(g.macros.get('MODEL'), lengths)
 
   vb = g.bindings_for('vocabularies.VocabularyConfig')
   kw = {}
@@ -187,14 +227,13 @@ class InferenceModel:
     self.sequence_length = lengths
     self.inputs_length = lengths['inputs']
     self.targets_length = lengths['targets']
+    # None: the no-context DiffusionModel (network.Transformer), as in the reference
     self.targets_context_length = lengths.get('targets_context', None)
-    if self.targets_context_length is None:
-      raise NotImplementedError(
-          'the no-context DiffusionModel (gin/models/diffusion/basic) is outside the built '
-          'path; use a context config (TASK_FEATURE_LENGTHS with targets_context)')
     self.audio_codec = audio_codecs.MelGAN()
     self.codec = codec
     self.model = _Model(t5, diff, self.audio_codec)
+    if self.targets_context_length is None:
+      self.model.FEATURE_CONVERTER_CLS = _NoContextFeatureConverterSpec
     self._engine: Optional[engine.Engine] = None
     self._device_index = device
     self._params = params
@@ -203,24 +242,45 @@ class InferenceModel:
 
   # ---- reference properties ---------------------------------------------------
   @property
+  def has_context(self) -> bool:
+    """Whether the model takes a context (ContextDiffusionModel) or not (DiffusionModel)."""
+    return self.targets_context_length is not None
+
+  @property
   def input_shapes(self):
     shapes = {
         'encoder_input_tokens': (self.batch_size, self.inputs_length),
         'decoder_target_tokens': (self.batch_size, self.targets_length, self.audio_codec.n_dims),
-        'encoder_continuous_inputs':
-            (self.batch_size, self.targets_context_length, self.audio_codec.n_dims),
-        'encoder_continuous_mask': (self.batch_size, self.targets_context_length),
     }
+    if self.has_context:
+      shapes.update({
+          'encoder_continuous_inputs':
+              (self.batch_size, self.targets_context_length, self.audio_codec.n_dims),
+          'encoder_continuous_mask': (self.batch_size, self.targets_context_length),
+      })
+    if 'decoder_input_tokens' in self.model.FEATURE_CONVERTER_CLS.MODEL_FEATURES:
+      shapes['decoder_input_tokens'] = shapes['decoder_target_tokens']
     return shapes
 
   @property
   def input_types(self):
-    return {
+    types = {
         'encoder_input_tokens': np.int32,
         'decoder_target_tokens': np.float32,
-        'encoder_continuous_inputs': np.float32,
-        'encoder_continuous_mask': np.int32,
     }
+    if self.has_context:
+      types.update({
+          'encoder_continuous_inputs': np.float32,
+          'encoder_continuous_mask': np.int32,
+      })
+    if 'decoder_input_tokens' in self.model.FEATURE_CONVERTER_CLS.MODEL_FEATURES:
+      types['decoder_input_tokens'] = types['decoder_target_tokens']
+    return types
+
+  def _encoder_inputs(self):
+    """The batch keys the engine's encode reads."""
+    return ('encoder_input_tokens', 'encoder_continuous_inputs',
+            'encoder_continuous_mask') if self.has_context else ('encoder_input_tokens',)
 
   @property
   def step(self):
@@ -258,9 +318,8 @@ class InferenceModel:
       eng.load_weights(self._restore_from_checkpoint())
       self._params = None  # the engine holds the packed copy
       dev = eng.device
-      for name, shape in self.input_shapes.items():
-        if name == 'decoder_target_tokens':
-          continue
+      for name in self._encoder_inputs():
+        shape = self.input_shapes[name]
         dt = torch.int32 if self.input_types[name] == np.int32 else torch.float32
         self._pinned[name] = torch.empty(shape, dtype=dt).pin_memory()
         self._dev[name] = torch.empty(shape, dtype=dt, device=dev)
@@ -274,8 +333,8 @@ class InferenceModel:
   def engine(self) -> engine.Engine:
     return self._get_engine()
 
-  def predict_on_device(self, tokens: torch.Tensor, ctx_features: torch.Tensor,
-                        ctx_mask: torch.Tensor, seed: int = 0,
+  def predict_on_device(self, tokens: torch.Tensor, ctx_features: Optional[torch.Tensor],
+                        ctx_mask: Optional[torch.Tensor], seed: int = 0,
                         init_z: Optional[torch.Tensor] = None,
                         noise: Optional[torch.Tensor] = None,
                         seeds: Optional[Sequence[int]] = None) -> torch.Tensor:
@@ -285,7 +344,8 @@ class InferenceModel:
     seeds: one seed per row; row b then draws its noise from seeds[b] alone, i.e. comes out as
     predict_on_device(row b, seed=seeds[b]) at batch 1 would draw it (Engine.sample_rows), so
     unrelated segments (e.g. of different songs) can share a batch.  `seed` is then unused, and
-    injected init_z / noise are not accepted."""
+    injected init_z / noise are not accepted.  A no-context model takes None for ctx_features and
+    ctx_mask."""
     eng = self._get_engine()
     b = tokens.shape[0]
     if b > self.batch_size:
@@ -294,8 +354,14 @@ class InferenceModel:
       raise ValueError('per-row seeds draw their own noise: init_z / noise cannot be injected')
     if seeds is not None and len(seeds) != b:
       raise ValueError(f'{len(seeds)} seeds for a batch of {b}')
-    eng.encode(tokens.to(torch.int32).contiguous(), ctx_features.to(torch.float32).contiguous(),
-               ctx_mask.to(torch.int32).contiguous())
+    if self.has_context:
+      if ctx_features is None or ctx_mask is None:
+        raise ValueError('this model takes a context: ctx_features and ctx_mask are required')
+      ctx_features = ctx_features.to(torch.float32).contiguous()
+      ctx_mask = ctx_mask.to(torch.int32).contiguous()
+    elif ctx_features is not None or ctx_mask is not None:
+      raise ValueError('the no-context model takes no ctx_features / ctx_mask (pass None)')
+    eng.encode(tokens.to(torch.int32).contiguous(), ctx_features, ctx_mask)
     if seeds is not None:
       return eng.sample_rows(seeds)
     return eng.sample(init_z, noise, seed=seed).clone()
@@ -303,14 +369,16 @@ class InferenceModel:
   def predict(self, batch: Mapping[str, np.ndarray], seed: int = 0,
               init_z: Optional[np.ndarray] = None, noise: Optional[np.ndarray] = None
               ) -> Tuple[np.ndarray, np.ndarray]:
-    """Host numpy batch in -> (pred_mel [B, targets, n_dims] in feature units, zeros [B])."""
+    """Host numpy batch in -> (pred_mel [B, targets, n_dims] in feature units, zeros [B]).
+    A no-context model reads encoder_input_tokens only and ignores the other keys, as the
+    reference's DiffusionModel.predict_batch_with_aux does (models.py:149-205)."""
     eng = self._get_engine()
     dev = eng.device
     b = int(np.asarray(batch['encoder_input_tokens']).shape[0])
     if b > self.batch_size:
       raise ValueError(f'batch of {b} exceeds batch_size={self.batch_size}')
     want = self.input_shapes
-    for name in ('encoder_input_tokens', 'encoder_continuous_inputs', 'encoder_continuous_mask'):
+    for name in self._encoder_inputs():
       arr = np.asarray(batch[name])
       if tuple(arr.shape[1:]) != tuple(want[name][1:]):
         raise ValueError(f'{name}: shape {arr.shape} does not match {want[name]}')
@@ -322,8 +390,11 @@ class InferenceModel:
         want['decoder_target_tokens'][1:]):
       raise ValueError('decoder_target_tokens: only its shape is used and it must be '
                        f'{want["decoder_target_tokens"]}')
-    eng.encode(self._dev['encoder_input_tokens'][:b], self._dev['encoder_continuous_inputs'][:b],
-               self._dev['encoder_continuous_mask'][:b])
+    if self.has_context:
+      eng.encode(self._dev['encoder_input_tokens'][:b], self._dev['encoder_continuous_inputs'][:b],
+                 self._dev['encoder_continuous_mask'][:b])
+    else:
+      eng.encode(self._dev['encoder_input_tokens'][:b], None, None)
     z0 = None if init_z is None else torch.from_numpy(
         np.ascontiguousarray(init_z, dtype=np.float32)).to(dev)
     nz = None if noise is None else torch.from_numpy(

@@ -19,6 +19,12 @@ audio without the absent vocoder, and `save_audio` writes it as a 16-bit WAV fil
 `synthesize_songs` runs several such chains at once: each round puts the next segment of every
 active song into one batch, one song per row, and every row draws its noise from its own song's
 seed (`InferenceModel.predict_on_device(..., seeds=)`), so a song comes out as it would alone.
+
+A model without a context (the reference's no-context `DiffusionModel`, lengths without
+`targets_context`) has no chain: a song's segments do not depend on each other, and the
+reference's loop predicts each one on its own with the song's seed (evaluation.py:179-210).  Both
+drivers then run every segment of every song as an independent batch row (`batch_segments`),
+`batch_size` rows per round, so a 12-segment song takes 2 rounds at batch 8 instead of 12 calls.
 """
 
 from __future__ import annotations
@@ -36,6 +42,21 @@ from music_spectrogram_diffusion_b200 import audio_codecs, midi_file, midi_token
 # predict_rows(tokens [R, inputs], ctx [R, context, n_dims], mask [R, context], seeds: R ints)
 #   -> mel [R, targets, n_dims]; row r must depend on row r of the inputs and seeds[r] only
 PredictRows = Callable[[torch.Tensor, torch.Tensor, torch.Tensor, Sequence[int]], torch.Tensor]
+# predict_segments(tokens [R, inputs], seeds: R ints) -> mel [R, targets, n_dims] of a model
+#   without a context; row r must depend on row r of the tokens and seeds[r] only
+PredictSegments = Callable[[torch.Tensor, Sequence[int]], torch.Tensor]
+
+
+def has_context(model) -> bool:
+  """Whether the model conditions a segment on a context (ContextDiffusionModel: its lengths have
+  `targets_context`) or not (DiffusionModel)."""
+  return 'targets_context' in model.sequence_length
+
+
+def _refuse_context(model, what: Optional[str]) -> None:
+  if what is not None:
+    raise ValueError(f'{what}: this model has no context (its TASK_FEATURE_LENGTHS '
+                     f'{dict(model.sequence_length)} lack targets_context)')
 
 
 def event_vocabulary_of(model) -> midi_tokens.EventVocabulary:
@@ -183,7 +204,17 @@ def synthesize_song(model, notes: np.ndarray, seed: int = 0, always_mask_context
 
   Returns {'full_pred_encoded': f32 [segments * targets_length, n_dims] in feature units,
   'num_frames': frames that belong to the song, 'tokens': the per-segment model inputs,
-  'model_timing': {...}} -- the same keys `beam/evaluation.py` yields for this part."""
+  'model_timing': {...}} -- the same keys `beam/evaluation.py` yields for this part.
+
+  A model without a context runs the song's segments as independent rows through
+  `synthesize_songs` (each as predict(segment, seed) computes it at batch 1, up to the kernels'
+  batch-size dependent rounding; bit for bit at batch_size 1); context_audio and
+  always_mask_context are refused for it."""
+  if not has_context(model):
+    _refuse_context(model, 'context_audio' if context_audio is not None else
+                    'always_mask_context' if always_mask_context else None)
+    results, _ = synthesize_songs(model, [notes], [seed], max_segments=max_segments)
+    return results[0]
   ac = model.audio_codec
   lengths = model.sequence_length
   toks, nseg = _tokenize(model, notes, max_segments)
@@ -299,6 +330,42 @@ def chain_songs(predict_rows: PredictRows, token_segments: Sequence[torch.Tensor
   return [torch.cat(o, dim=1) if o else empty for o in outs], rounds
 
 
+def batch_segments(predict_segments: PredictSegments, token_segments: Sequence[torch.Tensor],
+                   slots: int, n_dims: int, device: torch.device, seeds: Sequence[int]
+                   ) -> Tuple[List[torch.Tensor], List[Dict[str, Any]]]:
+  """Synthesis of several songs with a model without a context (the scheduling core of
+  `synthesize_songs` for it): no segment depends on another, so every segment of every song is an
+  independent row.  The rows -- song 0's segments in order, then song 1's, ... -- are packed in
+  that order into rounds of `slots` rows (the last one may be shorter), and each row draws its
+  noise from its song's seed.
+
+  token_segments[s]: int32 [n_segments_s, inputs_length].  Returns the same as `chain_songs`: (mel
+  [1, n_segments_s * frames, n_dims] per song, rounds), rounds[k] = {'rows': [(song, segment),
+  ...], 'seconds': host wall time of the round, synchronised with the device when the output is
+  a CUDA tensor}."""
+  if slots < 1:
+    raise ValueError(f'slots={slots} must be positive')
+  if len(seeds) != len(token_segments):
+    raise ValueError(f'{len(seeds)} seeds for {len(token_segments)} songs')
+  rows = [(s, k) for s, segs in enumerate(token_segments) for k in range(len(segs))]
+  outs: List[List[torch.Tensor]] = [[] for _ in token_segments]
+  rounds: List[Dict[str, Any]] = []
+  for first in range(0, len(rows), slots):
+    part = rows[first:first + slots]
+    toks = torch.stack([token_segments[s][k] for s, k in part]).to(device, torch.int32)
+    if toks.is_cuda:
+      torch.cuda.synchronize(device)
+    tick = time.time()
+    mel = predict_segments(toks, [seeds[s] for s, _ in part])
+    if mel.is_cuda:
+      torch.cuda.synchronize(mel.device)
+    rounds.append({'rows': part, 'seconds': time.time() - tick})
+    for r, (s, _) in enumerate(part):
+      outs[s].append(mel[r:r + 1])
+  empty = torch.zeros(1, 0, n_dims, dtype=torch.float32, device=device)
+  return [torch.cat(o, dim=1) if o else empty for o in outs], rounds
+
+
 def synthesize_songs(model, songs: Sequence[np.ndarray], seeds: Optional[Sequence[int]] = None,
                      always_mask_context: bool = False, max_segments: Optional[int] = None,
                      context_audios: Optional[Sequence[Any]] = None
@@ -310,6 +377,10 @@ def synthesize_songs(model, songs: Sequence[np.ndarray], seeds: Optional[Sequenc
   context_audios: one recording or None per song, as synthesize_song's context_audio; the
   recordings are encoded on the device and stay there.
 
+  A model without a context runs every segment of every song as an independent row instead
+  (`batch_segments`): model.batch_size rows per round, each segment as `predict(segment, seed)`
+  of its song computes it; context_audios and always_mask_context are refused for it.
+
   Returns (one dict per song with synthesize_song's keys, aggregate): model_timing of a song is
   the mean wall time of the rounds that carried its segments after its first; aggregate =
   {'rounds', 'segments', 'wall_seconds' (sum of the round times), 'audio_seconds',
@@ -318,6 +389,9 @@ def synthesize_songs(model, songs: Sequence[np.ndarray], seeds: Optional[Sequenc
     seeds = [0] * len(songs)
   if len(seeds) != len(songs):
     raise ValueError(f'{len(seeds)} seeds for {len(songs)} songs')
+  if not has_context(model):
+    _refuse_context(model, 'context_audios' if context_audios is not None else
+                    'always_mask_context' if always_mask_context else None)
   if context_audios is not None and len(context_audios) != len(songs):
     raise ValueError(f'{len(context_audios)} context recordings for {len(songs)} songs')
   if always_mask_context and context_audios is not None and any(
@@ -326,21 +400,26 @@ def synthesize_songs(model, songs: Sequence[np.ndarray], seeds: Optional[Sequenc
   ac = model.audio_codec
   lengths = model.sequence_length
   device = model.engine.device
-  primers = None if context_audios is None else [
-      None if a is None else audio_context(model, a, device) for a in context_audios]
   tokenized = [_tokenize(model, notes, max_segments) for notes in songs]
   segs = [torch.from_numpy(np.ascontiguousarray(t.tokens[:n], dtype=np.int32)).to(device)
           for t, n in tokenized]
-  mels, rounds = chain_songs(
-      lambda toks, ctx, mask, row_seeds: model.predict_on_device(toks, ctx, mask, seeds=row_seeds),
-      segs, model.batch_size, lengths.get('targets_context') or 0, ac.n_dims, device,
-      [int(s) for s in seeds], always_mask_context, primers)
+  if has_context(model):
+    primers = None if context_audios is None else [
+        None if a is None else audio_context(model, a, device) for a in context_audios]
+    mels, rounds = chain_songs(
+        lambda toks, ctx, mask, row_seeds: model.predict_on_device(toks, ctx, mask, seeds=row_seeds),
+        segs, model.batch_size, lengths.get('targets_context') or 0, ac.n_dims, device,
+        [int(s) for s in seeds], always_mask_context, primers)
+  else:
+    mels, rounds = batch_segments(
+        lambda toks, row_seeds: model.predict_on_device(toks, None, None, seeds=row_seeds),
+        segs, model.batch_size, ac.n_dims, device, [int(s) for s in seeds])
   seconds_per_chunk = lengths['targets'] * (ac.hop_size / ac.sample_rate)
   later: List[List[float]] = [[] for _ in songs]
   for rd in rounds:
-    for s, k in rd['rows']:
-      if k != 0:
-        later[s].append(rd['seconds'])
+    # each round once per song, however many of the song's segments it carried
+    for s in {s for s, k in rd['rows'] if k != 0}:
+      later[s].append(rd['seconds'])
   results = []
   for s, ((toks, nseg), mel) in enumerate(zip(tokenized, mels)):
     per_chunk = float(np.mean(later[s])) if later[s] else float('nan')

@@ -1,9 +1,12 @@
-"""Parameter tree of ContinuousContextTransformer: names, shapes, synthetic init.
+"""Parameter tree of ContinuousContextTransformer (or, without a context, Transformer): names,
+shapes, synthetic init.
 
 Names follow the flax tree the reference creates (SURVEY App. B):
   setup() attribute names   msd/models/diffusion/network.py:530-535
   layer / norm / dense names  network.py:127-152, 174-252, 278-301, 321-355,
                               380-456; msd/layers.py:262-264, 371-377, 485-508
+  no-context Transformer      network.py:460-468: token encoder `encoder`, no continuous
+                              encoder, one cross-attention source (`..._0` only)
 A real T5X checkpoint flattens to exactly these '/'-joined keys under
 ``target/`` (read by ``t5x_checkpoint.py``); the tree can also be synthesised
 (no checkpoint is available offline) or loaded from an ``.npz``.
@@ -12,7 +15,7 @@ A real T5X checkpoint flattens to exactly these '/'-joined keys under
 from __future__ import annotations
 
 import math
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
@@ -40,15 +43,18 @@ def _mlp(prefix: str, d: int, f: int, n_act: int) -> List[Tuple[str, Tuple[int, 
 
 
 def param_shapes(cfg: T5Config, inputs_length: int, targets_length: int,
-                 context_length: int, n_dims: int = 128
+                 context_length: Optional[int], n_dims: int = 128
                  ) -> List[Tuple[str, Tuple[int, ...]]]:
-  """Ordered (name, shape) list of every parameter on the inference path."""
+  """Ordered (name, shape) list of every parameter on the inference path.  context_length 0 or
+  None: the no-context network.Transformer tree."""
   d, hh, f = cfg.emb_dim, cfg.num_heads * cfg.head_dim, cfg.mlp_dim
   na = len(cfg.mlp_activations)
+  ctx = bool(context_length)
+  tok = 'token_encoder' if ctx else 'encoder'
   s: List[Tuple[str, Tuple[int, ...]]] = []
-  s.append(('token_encoder/token_embedder/embedding', (cfg.vocab_size, d)))
-  s.append(('token_encoder/Embed_0/embedding', (inputs_length, d)))
-  for enc, _ in (('token_encoder', 0), ('continuous_encoder', 1)):
+  s.append((f'{tok}/token_embedder/embedding', (cfg.vocab_size, d)))
+  s.append((f'{tok}/Embed_0/embedding', (inputs_length, d)))
+  for enc in (tok, 'continuous_encoder') if ctx else (tok,):
     if enc == 'continuous_encoder':
       s.append(('continuous_encoder/input_proj/kernel', (n_dims, d)))
       s.append(('continuous_encoder/Embed_0/embedding', (context_length, d)))
@@ -69,7 +75,9 @@ def param_shapes(cfg: T5Config, inputs_length: int, targets_length: int,
     s.append((f'{p}/FiLMLayer_0/DenseGeneral_0/kernel', (4 * d, 2 * d)))
     s += _attention(f'{p}/self_attention', d, hh)
     s.append((f'{p}/pre_cross_attention_layer_norm/scale', (d,)))
-    if cfg.decoder_cross_attend_style == 'concat_encodings':
+    # one attention per source for sum_cross_attends (network.py:199-216): without a context
+    # there is one source and either style has only `_0`
+    if cfg.decoder_cross_attend_style == 'concat_encodings' or not ctx:
       s += _attention(f'{p}/MultiHeadDotProductAttention_0', d, hh)
     else:
       s += _attention(f'{p}/MultiHeadDotProductAttention_0', d, hh)
@@ -101,7 +109,7 @@ def _sinusoidal(max_len: int, features: int, rng: np.random.Generator) -> np.nda
 
 
 def synthetic_params(cfg: T5Config, inputs_length: int = 2048,
-                     targets_length: int = 256, context_length: int = 256,
+                     targets_length: int = 256, context_length: Optional[int] = 256,
                      n_dims: int = 128, seed: int = 0) -> ParamDict:
   """Seeded random-init tree with the reference's initialiser statistics.
 
@@ -131,7 +139,7 @@ def synthetic_params(cfg: T5Config, inputs_length: int = 2048,
 
 
 def check_params(params: ParamDict, cfg: T5Config, inputs_length: int, targets_length: int,
-                 context_length: int, n_dims: int = 128) -> None:
+                 context_length: Optional[int], n_dims: int = 128) -> None:
   """Raises if a restored tree lacks a parameter of the inference path or has a wrong shape
   (the reference fails inside t5x's restore with a shape-mismatch error, inference.py:171-181).
   Extra entries (optimizer slots, unrelated modules) are ignored."""
