@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define MSD_B200_ABI_VERSION 6
+#define MSD_B200_ABI_VERSION 7
 
 typedef struct msd_ctx msd_ctx;
 
@@ -254,62 +254,122 @@ int msd_op_attention_f32(const float* q, const float* k, const float* v, const i
                          int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, float* out,
                          void* stream);
 
-/* The attention kernel on caller-owned device buffers, launched the way the engine launches it
- * (views into fused / cached buffers).  precision 0: bf16 q / k / v and the tensor-core kernel;
- * 1: fp32 q / k / v and the fp32 kernel.
- *   q / k / v   element offset + leading dimension (elements); head h reads columns h*64 .. +64 of
- *               the view.  Q rows [nb * Lq]; K / V row of batch b, key j: b * kv_batch_rows +
- *               kv_row0 + j (kv_batch_rows 0 = Lk).  k and v may be the same buffer.
- *   key_mask    int32 [nb, mask_len] (> 0 = attend) or NULL; packed to mask_len / 32 words per row,
- *               the attention reads words [mask_word0, mask_word0 + Lk / 32) of each row.
- *   kv_static   bf16 mode: K / V and the mask are read ahead of the programmatic-dependency wait.
- *               The hook completes all prior work on the stream, then rewrites the Q view (same
- *               values) with a kernel of its own and launches the attention right behind it.
- *   out         bf16; head h of row r written at out[o_col + r * o_ld + h*64 ..] (precision 0), or
- *               as [hi | lo | hi] at out[o_col + r * 3 * o_ld + {0, o_ld, 2 o_ld} + h*64 ..]
- *               (precision 1: o_ld is the width of one third).  Nothing else is written.
- *   part_o / part_ml  split-KV workspace for up to 12 splits: f32 [nb * Lq * heads * 12 * 64] and
- *               [nb * Lq * heads * 12 * 2].
- *   splits      0 = automatic, else forced (<= 12); tail (bf16 only): > 0 moves the last `tail`
- *               key blocks of an unsplit 128-key launch to a second CTA, 0 = none.
- * The key-block size follows MSD_ATTN_BKV as in the engine.  Synchronises the stream. */
-int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq, const void* k,
-                          int64_t k_off, int32_t ldk, const void* v, int64_t v_off, int32_t ldv,
-                          int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32_t kv_batch_rows,
-                          int32_t kv_row0, const int32_t* key_mask, int32_t mask_len,
-                          int32_t mask_word0, int32_t kv_static, void* out, int64_t o_col,
-                          int32_t o_ld, float* part_o, float* part_ml, int32_t splits, int32_t tail,
-                          void* stream);
+/* One attention launch on caller-owned device buffers, described the way the engine launches it
+ * (views into fused / cached buffers).  Every pointer is a device pointer. */
+typedef struct msd_attention_view_args {
+  int32_t precision;        /* 0: bf16 q / k / v and the tensor-core kernel; 1: fp32 q / k / v and
+                               the fp32 kernel */
+  void* q;                  /* q / k / v: element offset + leading dimension (elements); head h
+                               reads columns h*64 .. +64 of the view.  Q rows [nb * Lq]; K / V row
+                               of batch b, key j: b * kv_batch_rows + kv_row0 + j.  k and v may be
+                               the same buffer */
+  int64_t q_off;
+  int32_t ldq;
+  const void* k;
+  int64_t k_off;
+  int32_t ldk;
+  const void* v;
+  int64_t v_off;
+  int32_t ldv;
+  int32_t nb, heads, Lq, Lk;
+  int32_t kv_batch_rows;    /* 0 = Lk */
+  int32_t kv_row0;
+  const int32_t* key_mask;  /* int32 [nb, mask_len] (> 0 = attend) or NULL; packed to mask_len / 32
+                               words per row, the attention reads words [mask_word0, mask_word0 +
+                               Lk / 32) of each row */
+  int32_t mask_len;
+  int32_t mask_word0;
+  int32_t kv_static;        /* bf16 mode: K / V and the mask are read ahead of the programmatic-
+                               dependency wait.  The hook completes all prior work on the stream,
+                               then rewrites the Q view (same values) with a kernel of its own and
+                               launches the attention right behind it */
+  void* out;                /* bf16; head h of row r written at out[o_col + r * o_ld + h*64 ..]
+                               (precision 0), or as [hi | lo | hi] at out[o_col + r * 3 * o_ld +
+                               {0, o_ld, 2 o_ld} + h*64 ..] (precision 1: o_ld is the width of one
+                               third).  Nothing else is written */
+  int64_t o_col;
+  int32_t o_ld;
+  float* part_o;            /* part_o / part_ml: split-KV workspace for up to 12 splits: f32
+                               [nb * Lq * heads * 12 * 64] and [nb * Lq * heads * 12 * 2] */
+  float* part_ml;
+  int32_t splits;           /* 0 = automatic, else forced (<= 12) */
+  int32_t tail;             /* bf16 only: > 0 moves the last `tail` key blocks of an unsplit 128-key
+                               launch to a second CTA, 0 = none */
+} msd_attention_view_args;
 
-/* The GEMM on caller-owned device buffers, launched with every argument the engine's decoder sets
- * (views into fused buffers, step-indexed tables, deferred normalisation):
- *   a, b        bf16 operands as element offset + leading dimension: out = A[M, K] B[N, K]^T.
- *   epilogue    0 bf16, 1 f32, 2 f32 + resid, 3 gated GELU (bf16 [M, N / 2]), 4 f32 + position rows,
- *               5 gated GELU split [hi | lo | hi] (bf16 [M, 3 N / 2]), 6 deferred-normalisation
- *               producer (out == resid, f32 in place; see msd_op_dense_deferred_norm).
- *   block_n     0 = automatic, else 64 / 96 / 128 / 192 / 256; variant as in msd_op_dense_variant.
- *   out         f32 (epilogues 1, 2, 4, 6) or bf16 (0, 3, 5) at element offset out_off, row stride ldo;
- *               resid f32 at resid_off with the same ldo, or NULL.
- *   pos / pos_rows / pos_shift / dup_rows   epilogue 4, as in msd_op_dense_epilogue.
- *   step        device int32 diffusion step index the *_step_stride arguments multiply, or NULL.
- *   prep_*      epilogue 6: column gains g_lo (rows < prep_split_row) / g_hi at base + step * stride,
- *               bf16 operand written to prep_a [M, prep_lda], row sums of squares of each column tile
- *               t written to prep_ss[t * prep_ss_stride + row].
- *   rs_*        epilogues 0 / 3 (rs_ss_lo != NULL): row r's accumulator is scaled by
- *               rsqrt(inv_d * sum_{t < parts} ss[t * rs_ss_stride + r] + 1e-6), ss / parts = the _lo
- *               pair for r < rs_split_row, else the _hi pair; then rs_col_bias + step * stride is added.
- * *block_n_out (host, may be NULL) receives the tile width that ran: epilogue 6 writes N / width
- * partial sums per row.  The launch waits for all earlier work on the stream; synchronises it. */
-int msd_op_gemm_view(const void* a, int64_t a_off, int32_t lda, const void* b, int64_t b_off, int32_t ldb,
-                     int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n, int32_t variant,
-                     void* out, int64_t out_off, int32_t ldo, const float* resid, int64_t resid_off,
-                     const float* pos, int32_t pos_rows, const int32_t* pos_shift, int32_t dup_rows,
-                     const int32_t* step, const float* prep_g_lo, int64_t prep_g_lo_step_stride,
-                     const float* prep_g_hi, int64_t prep_g_hi_step_stride, int32_t prep_split_row,
-                     void* prep_a, int32_t prep_lda, float* prep_ss, int32_t prep_ss_stride,
-                     const float* rs_ss_lo, int32_t rs_parts_lo, const float* rs_ss_hi, int32_t rs_parts_hi,
-                     int32_t rs_split_row, int32_t rs_ss_stride, float rs_inv_d, const float* rs_col_bias,
-                     int64_t rs_bias_step_stride, int32_t* block_n_out, void* stream);
+/* The attention kernel as *args describes it (NULL args: -1).  The key-block size follows
+ * MSD_ATTN_BKV as in the engine.  Synchronises the stream. */
+int msd_op_attention_view(const msd_attention_view_args* args, void* stream);
+
+/* Epilogue 6 (deferred-normalisation producer) of msd_op_gemm_view: kernels.h GemmPrep. */
+typedef struct msd_gemm_prep {
+  const float* g_lo;          /* column gains of rows < split_row at g_lo + (*step) * g_lo_step_stride */
+  int64_t g_lo_step_stride;
+  const float* g_hi;          /* column gains of the other rows at g_hi + (*step) * g_hi_step_stride */
+  int64_t g_hi_step_stride;
+  int32_t split_row;
+  void* a;                    /* bf16 operand written to a [M, lda] */
+  int32_t lda;
+  float* ss;                  /* row sums of squares of each column tile t written to
+                                 ss[t * ss_stride + row] */
+  int32_t ss_stride;
+} msd_gemm_prep;
+
+/* The row scale of epilogues 0 / 3 of msd_op_gemm_view (applied when ss_lo != NULL): kernels.h
+ * GemmRowScale.  Row r's accumulator is scaled by rsqrt(inv_d * sum_{t < parts} ss[t * ss_stride +
+ * r] + 1e-6), ss / parts = the _lo pair for r < split_row, else the _hi pair; then col_bias +
+ * (*step) * bias_step_stride is added. */
+typedef struct msd_gemm_row_scale {
+  const float* ss_lo;
+  int32_t parts_lo;
+  const float* ss_hi;
+  int32_t parts_hi;
+  int32_t split_row;
+  int32_t ss_stride;
+  float inv_d;
+  const float* col_bias;      /* or NULL */
+  int64_t bias_step_stride;
+} msd_gemm_row_scale;
+
+/* One GEMM launch on caller-owned device buffers, with every argument the engine's decoder sets
+ * (views into fused buffers, step-indexed tables, deferred normalisation).  Every pointer is a
+ * device pointer. */
+typedef struct msd_gemm_view_args {
+  const void* a;              /* a, b: bf16 operands as element offset + leading dimension:
+                                 out = A[M, K] B[N, K]^T */
+  int64_t a_off;
+  int32_t lda;
+  const void* b;
+  int64_t b_off;
+  int32_t ldb;
+  int32_t M, N, K;
+  int32_t epilogue;           /* 0 bf16, 1 f32, 2 f32 + resid, 3 gated GELU (bf16 [M, N / 2]), 4 f32 +
+                                 position rows, 5 gated GELU split [hi | lo | hi] (bf16 [M, 3 N / 2]),
+                                 6 deferred-normalisation producer (out == resid, f32 in place; see
+                                 msd_op_dense_deferred_norm) */
+  int32_t block_n;            /* 0 = automatic, else 64 / 96 / 128 / 192 / 256 */
+  int32_t variant;            /* as in msd_op_dense_variant */
+  void* out;                  /* f32 (epilogues 1, 2, 4, 6) or bf16 (0, 3, 5) at element offset
+                                 out_off, row stride ldo */
+  int64_t out_off;
+  int32_t ldo;
+  const float* resid;         /* f32 at resid_off with the same ldo, or NULL */
+  int64_t resid_off;
+  const float* pos;           /* pos / pos_rows / pos_shift / dup_rows: epilogue 4, as in
+                                 msd_op_dense_epilogue */
+  int32_t pos_rows;
+  const int32_t* pos_shift;
+  int32_t dup_rows;
+  const int32_t* step;        /* device int32 diffusion step index the *_step_stride fields multiply,
+                                 or NULL */
+  msd_gemm_prep prep;         /* epilogue 6 */
+  msd_gemm_row_scale rs;      /* epilogues 0 / 3 */
+} msd_gemm_view_args;
+
+/* The GEMM as *args describes it (NULL args: -1).  *block_n_out (host, may be NULL) receives the
+ * tile width that ran: epilogue 6 writes N / width partial sums per row.  The launch waits for all
+ * earlier work on the stream; synchronises it. */
+int msd_op_gemm_view(const msd_gemm_view_args* args, int32_t* block_n_out, void* stream);
 
 /* The first decoder layer's deferred-normalisation prep (no GEMM produced its stream): a_out bf16
  * [rows, lda] = bf16(x * g), g at g + (*step) * g_step_stride; ss_out[row] = sum of x^2 over the
@@ -329,39 +389,72 @@ int msd_op_prep_rows(const float* x, const float* g, int64_t g_step_stride, cons
  * is refused (-1). */
 int msd_get_conditioning_tables(msd_ctx* ctx, float* film, float* gain, float* bias_qkv, float* bias_wi);
 
-/* The sampler kernel (one reverse step: guidance combine, x0, clip, DDPM / DDIM update, noise) on
- * caller-owned device buffers, with the fields the engine sets (no guidance split, no prefetch):
- *   eps       f32 [passes * n]: the model output of the conditional pass, then the unconditional one
- *   z         f32 [n], updated in place; z_split bf16 [n / n_dims, 3 n_dims] = [hi | lo | hi] of new z
- *   mel_out   f32 [n] or NULL: scale_to_features(z) written at step 0 only
- *   noise     f32 [num_steps, n] (row i read at step i) or NULL: generated from seed (rng_kind 0,
- *             Philox stream i + 1) or rng_keys [num_steps + 1][2] (rng_kind 1, row i + 1)
- *   coef      f32 [num_steps, 16] (msd_get_step_table layout)
- *   per_row   generated noise of row b = idx / n_row from row_seeds[b] (uint64, rng_kind 0) or
- *             row_keys + b * row_key_stride (rng_kind 1): n_row % 8 == 0, n < 2^32
- * step != NULL: the step index is read from that device int32 (one launch, per_row 0).
- * step == NULL: the graph's path.  A device RunArgs {noise, mel_out, seed, step = run_step, per_row}
- * is built, the kernel runs `launches` times behind each other (each launch advances the step), and
- * run_out[0] / run_out[1] (host) receive the RunArgs step and done counter found afterwards.
- * Refused (-1): null z / z_split / eps / coef, n not a positive multiple of n_dims (both multiples of
- * 4), passes other than 1 or 2, the jax stream without keys or with n % 8 != 0 or n >= 2^32, per-row
- * streams without their table or with n_row % 8 != 0 or n >= 2^32, and steps outside the table.
- * Synchronises the stream. */
-int msd_op_sampler_step(const float* eps, float* z, void* z_split, float* mel_out, const float* noise,
-                        const float* coef, int32_t num_steps, const int32_t* step, int64_t n, int32_t n_dims,
-                        int32_t passes, float cond_weight, int32_t clip_x0, int32_t ddim, float feat_min,
-                        float feat_max, uint64_t seed, int32_t rng_kind, const uint32_t* rng_keys,
-                        int64_t n_row, const uint32_t* row_keys, int64_t row_key_stride,
-                        const uint64_t* row_seeds, int32_t run_step, int32_t per_row, int32_t launches,
-                        int32_t* run_out, void* stream);
+/* The generated noise of msd_op_sampler_step and msd_op_init_z: one stream over the whole draw, or
+ * (per-row streams) one per row of n_row elements.  Tables are device pointers. */
+typedef struct msd_noise_streams {
+  uint64_t seed;                /* rng_kind 0: Philox stream i + 1 of seed at step i, stream 0 for z */
+  int32_t rng_kind;             /* 0 Philox, 1 jax.random threefry2x32 */
+  const uint32_t* rng_keys;     /* rng_kind 1: [num_steps + 1][2] keys, row i + 1 at step i, row 0
+                                   for z */
+  int64_t n_row;                /* per-row streams: element idx belongs to row b = idx / n_row */
+  const uint32_t* row_keys;     /* per-row streams, rng_kind 1: row b's key table, laid out as
+                                   rng_keys, at row_keys + b * row_key_stride */
+  int64_t row_key_stride;
+  const uint64_t* row_seeds;    /* per-row streams, rng_kind 0: row b's seed row_seeds[b] */
+} msd_noise_streams;
 
-/* The sampler's initial state: z f32 [n] = init_z (device copy) or, with init_z NULL, the draw of
- * Philox stream 0 of seed (rng_kind 0) or of key rng_keys[0..1] (rng_kind 1); n_row > 0: row b's own
- * draw from row_seeds[b] / rng_keys + b * row_key_stride.  z_split as in msd_op_sampler_step.
- * Synchronises the stream. */
-int msd_op_init_z(const float* init_z, float* z, void* z_split, int64_t n, int32_t n_dims, uint64_t seed,
-                  int32_t rng_kind, const uint32_t* rng_keys, int64_t n_row, int64_t row_key_stride,
-                  const uint64_t* row_seeds, void* stream);
+/* One reverse step of the sampler kernel on caller-owned device buffers, with the fields the engine
+ * sets (no guidance split, no prefetch).  Every pointer is a device pointer. */
+typedef struct msd_sampler_step_args {
+  const float* eps;             /* f32 [passes * n]: the model output of the conditional pass, then
+                                   the unconditional one */
+  float* z;                     /* f32 [n], updated in place */
+  void* z_split;                /* bf16 [n / n_dims, 3 n_dims] = [hi | lo | hi] of the new z */
+  float* mel_out;               /* f32 [n] or NULL: scale_to_features(z) written at step 0 only */
+  const float* noise;           /* f32 [num_steps, n] (row i read at step i) or NULL: generated from
+                                   streams */
+  const float* coef;            /* f32 [num_steps, 16] (msd_get_step_table layout) */
+  int32_t num_steps;
+  const int32_t* step;          /* non-NULL: the step index is read from this device int32 (one
+                                   launch, per_row 0).  NULL: the graph's RunArgs path */
+  int64_t n;
+  int32_t n_dims;
+  int32_t passes;
+  float cond_weight;
+  int32_t clip_x0;
+  int32_t ddim;
+  float feat_min;
+  float feat_max;
+  msd_noise_streams streams;    /* per-row streams need n_row % 8 == 0 and n < 2^32 */
+  int32_t run_step;             /* RunArgs path: the step of the first launch */
+  int32_t per_row;              /* RunArgs path: draw the generated noise from per-row streams */
+  int32_t launches;             /* RunArgs path: launches behind each other, each advancing the step */
+} msd_sampler_step_args;
+
+/* The sampler kernel (one reverse step: guidance combine, x0, clip, DDPM / DDIM update, noise) as
+ * *args describes it.  With args->step NULL (the graph's path), a device RunArgs {noise, mel_out,
+ * seed, step = run_step, per_row} is built, the kernel runs `launches` times, and run_out[0] /
+ * run_out[1] (host) receive the RunArgs step and done counter found afterwards.
+ * Refused (-1): NULL args, null z / z_split / eps / coef, n not a positive multiple of n_dims (both
+ * multiples of 4), passes other than 1 or 2, the jax stream without keys or with n % 8 != 0 or
+ * n >= 2^32, per-row streams without their table or with n_row % 8 != 0 or n >= 2^32, and steps
+ * outside the table.  Synchronises the stream. */
+int msd_op_sampler_step(const msd_sampler_step_args* args, int32_t* run_out, void* stream);
+
+/* The sampler's initial state.  Every pointer is a device pointer. */
+typedef struct msd_init_z_args {
+  const float* init_z;          /* f32 [n] copied to z, or NULL: the draw of streams */
+  float* z;                     /* f32 [n] */
+  void* z_split;                /* as in msd_sampler_step_args */
+  int64_t n;
+  int32_t n_dims;
+  msd_noise_streams streams;    /* Philox stream 0 of seed (rng_kind 0) or key rng_keys[0..1]
+                                   (rng_kind 1); n_row > 0: row b's own draw from row_seeds[b] /
+                                   row_keys + b * row_key_stride, both tables required */
+} msd_init_z_args;
+
+/* Writes the initial state as *args describes it (NULL args: -1).  Synchronises the stream. */
+int msd_op_init_z(const msd_init_z_args* args, void* stream);
 
 /* The encoder's context-feature front end (scale_features(clip=True), audio_codecs.py:166-174):
  * feat f32 [rows, n_dims] -> out_split bf16 [rows, 3 n_dims] = [hi | lo | hi] of

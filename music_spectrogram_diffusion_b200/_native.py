@@ -105,9 +105,85 @@ class MsdTensor(ctypes.Structure):
   ]
 
 
-# Every symbol include/msd_b200.h declares: (name, restype, argtypes)
+# The argument structs of the view hooks.  `__slots__ = ()` makes a misspelt field name raise instead
+# of becoming a plain Python attribute that the library never sees.
 _P = ctypes.c_void_p
 _I = ctypes.c_int32
+_L = ctypes.c_int64
+_F = ctypes.c_float
+
+
+class MsdAttentionViewArgs(ctypes.Structure):
+  """struct msd_attention_view_args (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('precision', _I), ('q', _P), ('q_off', _L), ('ldq', _I), ('k', _P), ('k_off', _L), ('ldk', _I),
+      ('v', _P), ('v_off', _L), ('ldv', _I), ('nb', _I), ('heads', _I), ('Lq', _I), ('Lk', _I),
+      ('kv_batch_rows', _I), ('kv_row0', _I), ('key_mask', _P), ('mask_len', _I), ('mask_word0', _I),
+      ('kv_static', _I), ('out', _P), ('o_col', _L), ('o_ld', _I), ('part_o', _P), ('part_ml', _P),
+      ('splits', _I), ('tail', _I),
+  ]
+
+
+class MsdGemmPrep(ctypes.Structure):
+  """struct msd_gemm_prep (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('g_lo', _P), ('g_lo_step_stride', _L), ('g_hi', _P), ('g_hi_step_stride', _L), ('split_row', _I),
+      ('a', _P), ('lda', _I), ('ss', _P), ('ss_stride', _I),
+  ]
+
+
+class MsdGemmRowScale(ctypes.Structure):
+  """struct msd_gemm_row_scale (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('ss_lo', _P), ('parts_lo', _I), ('ss_hi', _P), ('parts_hi', _I), ('split_row', _I), ('ss_stride', _I),
+      ('inv_d', _F), ('col_bias', _P), ('bias_step_stride', _L),
+  ]
+
+
+class MsdGemmViewArgs(ctypes.Structure):
+  """struct msd_gemm_view_args (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('a', _P), ('a_off', _L), ('lda', _I), ('b', _P), ('b_off', _L), ('ldb', _I),
+      ('M', _I), ('N', _I), ('K', _I), ('epilogue', _I), ('block_n', _I), ('variant', _I),
+      ('out', _P), ('out_off', _L), ('ldo', _I), ('resid', _P), ('resid_off', _L),
+      ('pos', _P), ('pos_rows', _I), ('pos_shift', _P), ('dup_rows', _I), ('step', _P),
+      ('prep', MsdGemmPrep), ('rs', MsdGemmRowScale),
+  ]
+
+
+class MsdNoiseStreams(ctypes.Structure):
+  """struct msd_noise_streams (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('seed', ctypes.c_uint64), ('rng_kind', _I), ('rng_keys', _P), ('n_row', _L), ('row_keys', _P),
+      ('row_key_stride', _L), ('row_seeds', _P),
+  ]
+
+
+class MsdSamplerStepArgs(ctypes.Structure):
+  """struct msd_sampler_step_args (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('eps', _P), ('z', _P), ('z_split', _P), ('mel_out', _P), ('noise', _P), ('coef', _P),
+      ('num_steps', _I), ('step', _P), ('n', _L), ('n_dims', _I), ('passes', _I), ('cond_weight', _F),
+      ('clip_x0', _I), ('ddim', _I), ('feat_min', _F), ('feat_max', _F), ('streams', MsdNoiseStreams),
+      ('run_step', _I), ('per_row', _I), ('launches', _I),
+  ]
+
+
+class MsdInitZArgs(ctypes.Structure):
+  """struct msd_init_z_args (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('init_z', _P), ('z', _P), ('z_split', _P), ('n', _L), ('n_dims', _I), ('streams', MsdNoiseStreams),
+  ]
+
+
+# Every symbol include/msd_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ('msd_last_error', ctypes.c_char_p, []),
     ('msd_abi_version', ctypes.c_int, []),
@@ -138,22 +214,12 @@ SYMBOLS = [
     ('msd_op_dense_deferred_norm', ctypes.c_int,
      [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _I, _I, _P, _P, _P]),
     ('msd_op_attention_f32', ctypes.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
-    ('msd_op_attention_view', ctypes.c_int,
-     [_I, _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _I, _I, _I, _I, _I, _I,
-      _P, _I, _I, _I, _P, ctypes.c_int64, _I, _P, _P, _I, _I, _P]),
-    ('msd_op_gemm_view', ctypes.c_int,
-     [_P, ctypes.c_int64, _I, _P, ctypes.c_int64, _I, _I, _I, _I, _I, _I, _I,
-      _P, ctypes.c_int64, _I, _P, ctypes.c_int64, _P, _I, _P, _I,
-      _P, _P, ctypes.c_int64, _P, ctypes.c_int64, _I, _P, _I, _P, _I,
-      _P, _I, _P, _I, _I, _I, ctypes.c_float, _P, ctypes.c_int64, ctypes.POINTER(_I), _P]),
+    ('msd_op_attention_view', ctypes.c_int, [ctypes.POINTER(MsdAttentionViewArgs), _P]),
+    ('msd_op_gemm_view', ctypes.c_int, [ctypes.POINTER(MsdGemmViewArgs), ctypes.POINTER(_I), _P]),
     ('msd_op_prep_rows', ctypes.c_int, [_P, _P, ctypes.c_int64, _P, _I, _I, _P, _I, _P, _P]),
     ('msd_get_conditioning_tables', ctypes.c_int, [_P, _P, _P, _P, _P]),
-    ('msd_op_sampler_step', ctypes.c_int,
-     [_P, _P, _P, _P, _P, _P, _I, _P, ctypes.c_int64, _I, _I, ctypes.c_float, _I, _I, ctypes.c_float,
-      ctypes.c_float, ctypes.c_uint64, _I, _P, ctypes.c_int64, _P, ctypes.c_int64, _P, _I, _I, _I,
-      ctypes.POINTER(_I), _P]),
-    ('msd_op_init_z', ctypes.c_int,
-     [_P, _P, _P, ctypes.c_int64, _I, ctypes.c_uint64, _I, _P, ctypes.c_int64, ctypes.c_int64, _P, _P]),
+    ('msd_op_sampler_step', ctypes.c_int, [ctypes.POINTER(MsdSamplerStepArgs), ctypes.POINTER(_I), _P]),
+    ('msd_op_init_z', ctypes.c_int, [ctypes.POINTER(MsdInitZArgs), _P]),
     ('msd_op_scale_split', ctypes.c_int,
      [_P, _P, ctypes.c_int64, _I, ctypes.c_float, ctypes.c_float, _P]),
     ('msd_op_audio_mel', ctypes.c_int, [_P, _I, ctypes.c_int64, _P, _P, _P, _P]),
@@ -166,7 +232,7 @@ SYMBOLS = [
      [_P, _I, ctypes.c_int64, _P, _P, _P, _P, ctypes.c_float, _I, _P]),
     ('msd_op_griffin_lim_istft', ctypes.c_int, [_P, _P, _I, ctypes.c_int64, _P, _P, _P]),
 ]
-ABI_VERSION = 6  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
+ABI_VERSION = 7  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
 
 _lib: Optional[ctypes.CDLL] = None
 

@@ -514,34 +514,30 @@ int msd_op_attention_f32(const float* q, const float* k, const float* v, const i
   return 0;
 }
 
-int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq, const void* k,
-                          int64_t k_off, int32_t ldk, const void* v, int64_t v_off, int32_t ldv,
-                          int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32_t kv_batch_rows,
-                          int32_t kv_row0, const int32_t* key_mask, int32_t mask_len,
-                          int32_t mask_word0, int32_t kv_static, void* out, int64_t o_col,
-                          int32_t o_ld, float* part_o, float* part_ml, int32_t splits, int32_t tail,
-                          void* stream) {
-  MSD_REQUIRE(q && k && v && out && part_o && part_ml, "msd_op_attention_view: null argument");
-  MSD_REQUIRE(precision == 0 || precision == 1, "msd_op_attention_view: precision must be 0 or 1");
-  MSD_REQUIRE(nb > 0 && heads > 0 && Lq > 0 && Lk > 0 && q_off >= 0 && k_off >= 0 && v_off >= 0 &&
-                  o_col >= 0 && kv_row0 >= 0 && kv_batch_rows >= 0,
+int msd_op_attention_view(const msd_attention_view_args* args, void* stream) {
+  MSD_REQUIRE(args && args->q && args->k && args->v && args->out && args->part_o && args->part_ml,
+              "msd_op_attention_view: null argument");
+  const msd_attention_view_args& a = *args;
+  MSD_REQUIRE(a.precision == 0 || a.precision == 1, "msd_op_attention_view: precision must be 0 or 1");
+  MSD_REQUIRE(a.nb > 0 && a.heads > 0 && a.Lq > 0 && a.Lk > 0 && a.q_off >= 0 && a.k_off >= 0 && a.v_off >= 0 &&
+                  a.o_col >= 0 && a.kv_row0 >= 0 && a.kv_batch_rows >= 0,
               "msd_op_attention_view: bad sizes or offsets");
-  MSD_REQUIRE(splits >= 0 && splits <= 12 && tail >= 0 && (precision == 0 || tail == 0),
+  MSD_REQUIRE(a.splits >= 0 && a.splits <= 12 && a.tail >= 0 && (a.precision == 0 || a.tail == 0),
               "msd_op_attention_view: splits must be in [0, 12], tail >= 0 (bf16 mode only)");
-  MSD_REQUIRE(!key_mask || (mask_len % 128 == 0 && mask_word0 >= 0 && mask_word0 % 4 == 0 &&
-                            mask_word0 + Lk / 32 <= mask_len / 32),
-              "msd_op_attention_view: mask words [%d, %d) outside rows of %d keys", mask_word0,
-              mask_word0 + Lk / 32, mask_len);
+  MSD_REQUIRE(!a.key_mask || (a.mask_len % 128 == 0 && a.mask_word0 >= 0 && a.mask_word0 % 4 == 0 &&
+                              a.mask_word0 + a.Lk / 32 <= a.mask_len / 32),
+              "msd_op_attention_view: mask words [%d, %d) outside rows of %d keys", a.mask_word0,
+              a.mask_word0 + a.Lk / 32, a.mask_len);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t es = precision ? 4 : 2;
-  const int width = heads * 64;
-  const long long rows_q = static_cast<long long>(nb) * Lq;
-  char* qv = static_cast<char*>(q) + q_off * es;
+  const size_t es = a.precision ? 4 : 2;
+  const int width = a.heads * 64;
+  const long long rows_q = static_cast<long long>(a.nb) * a.Lq;
+  char* qv = static_cast<char*>(a.q) + a.q_off * es;
   TempBufs tb;
   uint32_t* bits = nullptr;
-  if (key_mask) {
-    MSD_TRY(tb.get(&bits, static_cast<size_t>(nb) * (mask_len / 32)));
-    MSD_TRY(launch_mask_bits(key_mask, nb, mask_len, bits, st));
+  if (a.key_mask) {
+    MSD_TRY(tb.get(&bits, static_cast<size_t>(a.nb) * (a.mask_len / 32)));
+    MSD_TRY(launch_mask_bits(a.key_mask, a.nb, a.mask_len, bits, st));
   }
   // K, V and the mask must be complete before the attention starts (kv_static reads them ahead of
   // its dependency wait, as after the plain first launch of a diffusion step).  Q is then written
@@ -549,69 +545,62 @@ int msd_op_attention_view(int32_t precision, void* q, int64_t q_off, int32_t ldq
   // live predecessor, as in the step graph.
   char* stage = nullptr;
   MSD_TRY(tb.get(&stage, static_cast<size_t>(rows_q) * width * es));
-  MSD_CUDA_CHECK(cudaMemcpy2DAsync(stage, width * es, qv, ldq * es, width * es, rows_q,
+  MSD_CUDA_CHECK(cudaMemcpy2DAsync(stage, width * es, qv, a.ldq * es, width * es, rows_q,
                                    cudaMemcpyDeviceToDevice, st));
   MSD_CUDA_CHECK(cudaStreamSynchronize(st));
-  MSD_TRY(launch_copy_rows(stage, static_cast<long long>(width * es), qv, static_cast<long long>(ldq) * es,
+  MSD_TRY(launch_copy_rows(stage, static_cast<long long>(width * es), qv, static_cast<long long>(a.ldq) * es,
                            rows_q, static_cast<int>(width * es), st));
   AttnView view = {};
-  view.f32 = precision == 1;
-  view.Q = qv; view.ldq = ldq;
-  view.K = k; view.k_off = k_off; view.ldk = ldk;
-  view.V = v; view.v_off = v_off; view.ldv = ldv;
-  view.O = static_cast<bf16*>(out) + o_col; view.ldo = o_ld;
-  view.nbatch = nb; view.heads = heads; view.Lq = Lq; view.Lk = Lk;
-  view.mask_bits = bits ? bits + mask_word0 : nullptr; view.mask_stride_words = mask_len / 32;
-  view.part_o = part_o; view.part_ml = part_ml; view.max_splits = 12;
-  view.splits = splits; view.tail = tail;
-  view.kv_static = kv_static; view.kv_batch_rows = kv_batch_rows; view.kv_row0 = kv_row0;
+  view.f32 = a.precision == 1;
+  view.Q = qv; view.ldq = a.ldq;
+  view.K = a.k; view.k_off = a.k_off; view.ldk = a.ldk;
+  view.V = a.v; view.v_off = a.v_off; view.ldv = a.ldv;
+  view.O = static_cast<bf16*>(a.out) + a.o_col; view.ldo = a.o_ld;
+  view.nbatch = a.nb; view.heads = a.heads; view.Lq = a.Lq; view.Lk = a.Lk;
+  view.mask_bits = bits ? bits + a.mask_word0 : nullptr; view.mask_stride_words = a.mask_len / 32;
+  view.part_o = a.part_o; view.part_ml = a.part_ml; view.max_splits = 12;
+  view.splits = a.splits; view.tail = a.tail;
+  view.kv_static = a.kv_static; view.kv_batch_rows = a.kv_batch_rows; view.kv_row0 = a.kv_row0;
   MSD_TRY(launch_attention_view(view, st));
   MSD_CUDA_CHECK(cudaStreamSynchronize(st));
   return 0;
 }
 
-int msd_op_gemm_view(const void* a, int64_t a_off, int32_t lda, const void* b, int64_t b_off, int32_t ldb,
-                     int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n, int32_t variant,
-                     void* out, int64_t out_off, int32_t ldo, const float* resid, int64_t resid_off,
-                     const float* pos, int32_t pos_rows, const int32_t* pos_shift, int32_t dup_rows,
-                     const int32_t* step, const float* prep_g_lo, int64_t prep_g_lo_step_stride,
-                     const float* prep_g_hi, int64_t prep_g_hi_step_stride, int32_t prep_split_row,
-                     void* prep_a, int32_t prep_lda, float* prep_ss, int32_t prep_ss_stride,
-                     const float* rs_ss_lo, int32_t rs_parts_lo, const float* rs_ss_hi, int32_t rs_parts_hi,
-                     int32_t rs_split_row, int32_t rs_ss_stride, float rs_inv_d, const float* rs_col_bias,
-                     int64_t rs_bias_step_stride, int32_t* block_n_out, void* stream) {
-  MSD_REQUIRE(a && b && out, "msd_op_gemm_view: null argument");
-  MSD_REQUIRE(epilogue >= EPI_BF16 && epilogue <= EPI_RESID_PREP, "msd_op_gemm_view: unknown epilogue %d",
-              epilogue);
-  MSD_REQUIRE(a_off >= 0 && b_off >= 0 && out_off >= 0 && resid_off >= 0,
+int msd_op_gemm_view(const msd_gemm_view_args* args, int32_t* block_n_out, void* stream) {
+  MSD_REQUIRE(args && args->a && args->b && args->out, "msd_op_gemm_view: null argument");
+  const msd_gemm_view_args& v = *args;
+  MSD_REQUIRE(v.epilogue >= EPI_BF16 && v.epilogue <= EPI_RESID_PREP, "msd_op_gemm_view: unknown epilogue %d",
+              v.epilogue);
+  MSD_REQUIRE(v.a_off >= 0 && v.b_off >= 0 && v.out_off >= 0 && v.resid_off >= 0,
               "msd_op_gemm_view: negative offset");
-  const bool f32_out = epilogue == EPI_F32 || epilogue == EPI_RESID_F32 || epilogue == EPI_POS_F32 ||
-                       epilogue == EPI_RESID_PREP;
+  const bool f32_out = v.epilogue == EPI_F32 || v.epilogue == EPI_RESID_F32 || v.epilogue == EPI_POS_F32 ||
+                       v.epilogue == EPI_RESID_PREP;
   GemmArgs g;
   memset(&g, 0, sizeof(g));
-  g.A = static_cast<const bf16*>(a) + a_off; g.lda = lda;
-  g.B = static_cast<const bf16*>(b) + b_off; g.ldb = ldb;
-  g.M = M; g.N = N; g.K = K; g.epilogue = epilogue; g.block_n = block_n; g.variant = variant;
-  g.out = f32_out ? static_cast<void*>(static_cast<float*>(out) + out_off)
-                  : static_cast<void*>(static_cast<bf16*>(out) + out_off);
-  g.ldo = ldo;
-  g.resid = resid ? resid + resid_off : nullptr;
-  g.pos = pos; g.pos_rows = pos_rows; g.pos_shift = pos_shift; g.dup_rows = dup_rows;
-  g.step = step;
-  g.prep.g_lo = prep_g_lo; g.prep.g_lo_step_stride = prep_g_lo_step_stride;
-  g.prep.g_hi = prep_g_hi; g.prep.g_hi_step_stride = prep_g_hi_step_stride;
-  g.prep.split_row = prep_split_row;
-  g.prep.a = static_cast<bf16*>(prep_a); g.prep.lda = prep_lda;
-  g.prep.ss = prep_ss; g.prep.ss_stride = prep_ss_stride;
-  g.rs.ss_lo = rs_ss_lo; g.rs.parts_lo = rs_parts_lo; g.rs.ss_hi = rs_ss_hi; g.rs.parts_hi = rs_parts_hi;
-  g.rs.split_row = rs_split_row; g.rs.ss_stride = rs_ss_stride; g.rs.inv_d = rs_inv_d;
-  g.rs.col_bias = rs_col_bias; g.rs.bias_step_stride = rs_bias_step_stride;
-  MSD_REQUIRE(epilogue != EPI_RESID_PREP || g.prep.a != nullptr,
+  g.A = static_cast<const bf16*>(v.a) + v.a_off; g.lda = v.lda;
+  g.B = static_cast<const bf16*>(v.b) + v.b_off; g.ldb = v.ldb;
+  g.M = v.M; g.N = v.N; g.K = v.K; g.epilogue = v.epilogue; g.block_n = v.block_n; g.variant = v.variant;
+  g.out = f32_out ? static_cast<void*>(static_cast<float*>(v.out) + v.out_off)
+                  : static_cast<void*>(static_cast<bf16*>(v.out) + v.out_off);
+  g.ldo = v.ldo;
+  g.resid = v.resid ? v.resid + v.resid_off : nullptr;
+  g.pos = v.pos; g.pos_rows = v.pos_rows; g.pos_shift = v.pos_shift; g.dup_rows = v.dup_rows;
+  g.step = v.step;
+  g.prep.g_lo = v.prep.g_lo; g.prep.g_lo_step_stride = v.prep.g_lo_step_stride;
+  g.prep.g_hi = v.prep.g_hi; g.prep.g_hi_step_stride = v.prep.g_hi_step_stride;
+  g.prep.split_row = v.prep.split_row;
+  g.prep.a = static_cast<bf16*>(v.prep.a); g.prep.lda = v.prep.lda;
+  g.prep.ss = v.prep.ss; g.prep.ss_stride = v.prep.ss_stride;
+  g.rs.ss_lo = v.rs.ss_lo; g.rs.parts_lo = v.rs.parts_lo; g.rs.ss_hi = v.rs.ss_hi; g.rs.parts_hi = v.rs.parts_hi;
+  g.rs.split_row = v.rs.split_row; g.rs.ss_stride = v.rs.ss_stride; g.rs.inv_d = v.rs.inv_d;
+  g.rs.col_bias = v.rs.col_bias; g.rs.bias_step_stride = v.rs.bias_step_stride;
+  MSD_REQUIRE(v.epilogue != EPI_RESID_PREP || g.prep.a != nullptr,
               "msd_op_gemm_view: EPI_RESID_PREP needs prep_a");
-  MSD_REQUIRE(epilogue != EPI_POS_F32 || (pos != nullptr && pos_rows > 0),
+  MSD_REQUIRE(v.epilogue != EPI_POS_F32 || (v.pos != nullptr && v.pos_rows > 0),
               "msd_op_gemm_view: EPI_POS_F32 needs pos / pos_rows");
   const int bn = gemm_resolve_block_n(g);
-  MSD_REQUIRE(bn > 0, "msd_op_gemm_view: N=%d has no tile width (block_n %d, variant %d)", N, block_n, variant);
+  MSD_REQUIRE(bn > 0, "msd_op_gemm_view: N=%d has no tile width (block_n %d, variant %d)", v.N, v.block_n,
+              v.variant);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   g_pdl_skip_next = true;   // the operands were just written by the caller's own kernels
   MSD_TRY(launch_gemm(g, st));
@@ -631,44 +620,40 @@ int msd_op_prep_rows(const float* x, const float* g, int64_t g_step_stride, cons
   return 0;
 }
 
-int msd_op_sampler_step(const float* eps, float* z, void* z_split, float* mel_out, const float* noise,
-                        const float* coef, int32_t num_steps, const int32_t* step, int64_t n, int32_t n_dims,
-                        int32_t passes, float cond_weight, int32_t clip_x0, int32_t ddim, float feat_min,
-                        float feat_max, uint64_t seed, int32_t rng_kind, const uint32_t* rng_keys,
-                        int64_t n_row, const uint32_t* row_keys, int64_t row_key_stride,
-                        const uint64_t* row_seeds, int32_t run_step, int32_t per_row, int32_t launches,
-                        int32_t* run_out, void* stream) {
-  MSD_REQUIRE(eps && z && z_split && coef, "msd_op_sampler_step: null argument");
-  MSD_REQUIRE(n > 0 && n_dims > 0 && n % 4 == 0 && n_dims % 4 == 0 && n % n_dims == 0 && num_steps > 0,
+int msd_op_sampler_step(const msd_sampler_step_args* args, int32_t* run_out, void* stream) {
+  MSD_REQUIRE(args && args->eps && args->z && args->z_split && args->coef, "msd_op_sampler_step: null argument");
+  const msd_sampler_step_args& s = *args;
+  const msd_noise_streams& ns = s.streams;
+  MSD_REQUIRE(s.n > 0 && s.n_dims > 0 && s.n % 4 == 0 && s.n_dims % 4 == 0 && s.n % s.n_dims == 0 && s.num_steps > 0,
               "msd_op_sampler_step: n=%lld must be a positive multiple of n_dims=%d, both multiples of 4",
-              static_cast<long long>(n), n_dims);
-  MSD_REQUIRE(passes == 1 || passes == 2, "msd_op_sampler_step: passes must be 1 or 2 (got %d)", passes);
-  MSD_REQUIRE(rng_kind == 0 || rng_kind == 1, "msd_op_sampler_step: rng_kind must be 0 or 1");
-  MSD_REQUIRE(rng_kind == 0 || per_row || (rng_keys != nullptr && n % 8 == 0 && n < (1ll << 32)),
+              static_cast<long long>(s.n), s.n_dims);
+  MSD_REQUIRE(s.passes == 1 || s.passes == 2, "msd_op_sampler_step: passes must be 1 or 2 (got %d)", s.passes);
+  MSD_REQUIRE(ns.rng_kind == 0 || ns.rng_kind == 1, "msd_op_sampler_step: rng_kind must be 0 or 1");
+  MSD_REQUIRE(ns.rng_kind == 0 || s.per_row || (ns.rng_keys != nullptr && s.n % 8 == 0 && s.n < (1ll << 32)),
               "msd_op_sampler_step: the jax stream needs its key table and a draw of k*8 < 2^32 elements");
-  MSD_REQUIRE(!per_row || (n_row > 0 && n_row % 8 == 0 && n % n_row == 0 && n < (1ll << 32) &&
-                           (rng_kind == 0 ? row_seeds != nullptr : row_keys != nullptr)),
+  MSD_REQUIRE(!s.per_row || (ns.n_row > 0 && ns.n_row % 8 == 0 && s.n % ns.n_row == 0 && s.n < (1ll << 32) &&
+                             (ns.rng_kind == 0 ? ns.row_seeds != nullptr : ns.row_keys != nullptr)),
               "msd_op_sampler_step: per-row streams need rows of k*8 elements, n < 2^32 and the row table");
-  MSD_REQUIRE(step == nullptr || (!per_row && launches == 1),
+  MSD_REQUIRE(s.step == nullptr || (!s.per_row && s.launches == 1),
               "msd_op_sampler_step: per-row streams and several launches need the RunArgs path (step NULL)");
-  MSD_REQUIRE(step != nullptr || run_out != nullptr, "msd_op_sampler_step: the RunArgs path needs run_out");
+  MSD_REQUIRE(s.step != nullptr || run_out != nullptr, "msd_op_sampler_step: the RunArgs path needs run_out");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int first = run_step;
-  if (step != nullptr) MSD_CUDA_CHECK(cudaMemcpy(&first, step, sizeof(int), cudaMemcpyDeviceToHost));
-  MSD_REQUIRE(launches >= 1 && first < num_steps && first - launches + 1 >= 0,
-              "msd_op_sampler_step: %d launch(es) from step %d leave the table of %d steps", launches, first,
-              num_steps);
+  int first = s.run_step;
+  if (s.step != nullptr) MSD_CUDA_CHECK(cudaMemcpy(&first, s.step, sizeof(int), cudaMemcpyDeviceToHost));
+  MSD_REQUIRE(s.launches >= 1 && first < s.num_steps && first - s.launches + 1 >= 0,
+              "msd_op_sampler_step: %d launch(es) from step %d leave the table of %d steps", s.launches, first,
+              s.num_steps);
   SamplerArgs a;
   memset(&a, 0, sizeof(a));
-  a.eps = eps; a.z = z; a.z_split = static_cast<bf16*>(z_split); a.coef = coef;
-  a.n = n; a.n_dims = n_dims; a.passes = passes; a.cond_weight = cond_weight;
-  a.clip_x0 = clip_x0; a.ddim = ddim; a.feat_min = feat_min; a.feat_max = feat_max;
-  a.rng_kind = rng_kind; a.rng_keys = rng_keys;
-  a.n_row = n_row; a.row_keys = row_keys; a.row_key_stride = row_key_stride;
-  a.row_seeds = reinterpret_cast<const unsigned long long*>(row_seeds);
+  a.eps = s.eps; a.z = s.z; a.z_split = static_cast<bf16*>(s.z_split); a.coef = s.coef;
+  a.n = s.n; a.n_dims = s.n_dims; a.passes = s.passes; a.cond_weight = s.cond_weight;
+  a.clip_x0 = s.clip_x0; a.ddim = s.ddim; a.feat_min = s.feat_min; a.feat_max = s.feat_max;
+  a.rng_kind = ns.rng_kind; a.rng_keys = ns.rng_keys;
+  a.n_row = ns.n_row; a.row_keys = ns.row_keys; a.row_key_stride = ns.row_key_stride;
+  a.row_seeds = reinterpret_cast<const unsigned long long*>(ns.row_seeds);
   TempBufs tb;
-  if (step != nullptr) {
-    a.step = step; a.noise = noise; a.mel_out = mel_out; a.seed = seed;
+  if (s.step != nullptr) {
+    a.step = s.step; a.noise = s.noise; a.mel_out = s.mel_out; a.seed = ns.seed;
     g_pdl_skip_next = true;   // the inputs were just written by the caller's own kernels
     MSD_TRY(launch_sampler_step(a, st));
     MSD_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -676,13 +661,13 @@ int msd_op_sampler_step(const float* eps, float* z, void* z_split, float* mel_ou
   }
   RunArgs ra;
   memset(&ra, 0, sizeof(ra));
-  ra.noise = noise; ra.mel_out = mel_out; ra.seed = seed; ra.step = run_step; ra.per_row = per_row;
+  ra.noise = s.noise; ra.mel_out = s.mel_out; ra.seed = ns.seed; ra.step = s.run_step; ra.per_row = s.per_row;
   MSD_TRY(tb.get(&a.run, 1));
   MSD_CUDA_CHECK(cudaMemcpyAsync(a.run, &ra, sizeof(ra), cudaMemcpyHostToDevice, st));
   // the first launch follows the upload; the next ones are PDL launches behind the previous step's
   // sampler kernel, which is what the step graph's first kernel sees
   g_pdl_skip_next = true;
-  for (int i = 0; i < launches; ++i) MSD_TRY(launch_sampler_step(a, st));
+  for (int i = 0; i < s.launches; ++i) MSD_TRY(launch_sampler_step(a, st));
   MSD_CUDA_CHECK(cudaMemcpyAsync(&ra, a.run, sizeof(ra), cudaMemcpyDeviceToHost, st));
   MSD_CUDA_CHECK(cudaStreamSynchronize(st));
   run_out[0] = ra.step;
@@ -690,17 +675,19 @@ int msd_op_sampler_step(const float* eps, float* z, void* z_split, float* mel_ou
   return 0;
 }
 
-int msd_op_init_z(const float* init_z, float* z, void* z_split, int64_t n, int32_t n_dims, uint64_t seed,
-                  int32_t rng_kind, const uint32_t* rng_keys, int64_t n_row, int64_t row_key_stride,
-                  const uint64_t* row_seeds, void* stream) {
-  MSD_REQUIRE(z && z_split, "msd_op_init_z: null argument");
-  MSD_REQUIRE(n > 0 && n_dims > 0 && n % 4 == 0 && n_dims % 4 == 0 && n % n_dims == 0,
+int msd_op_init_z(const msd_init_z_args* args, void* stream) {
+  MSD_REQUIRE(args && args->z && args->z_split, "msd_op_init_z: null argument");
+  const msd_init_z_args& a = *args;
+  const msd_noise_streams& ns = a.streams;
+  MSD_REQUIRE(a.n > 0 && a.n_dims > 0 && a.n % 4 == 0 && a.n_dims % 4 == 0 && a.n % a.n_dims == 0,
               "msd_op_init_z: n=%lld must be a positive multiple of n_dims=%d, both multiples of 4",
-              static_cast<long long>(n), n_dims);
-  MSD_REQUIRE(rng_kind == 0 || rng_kind == 1, "msd_op_init_z: rng_kind must be 0 or 1");
+              static_cast<long long>(a.n), a.n_dims);
+  MSD_REQUIRE(ns.rng_kind == 0 || ns.rng_kind == 1, "msd_op_init_z: rng_kind must be 0 or 1");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  MSD_TRY(launch_init_z(init_z, z, static_cast<bf16*>(z_split), n, n_dims, seed, st, rng_kind, rng_keys, n_row,
-                        row_key_stride, reinterpret_cast<const unsigned long long*>(row_seeds)));
+  // launch_init_z reads the per-row key tables from its rng_keys argument
+  MSD_TRY(launch_init_z(a.init_z, a.z, static_cast<bf16*>(a.z_split), a.n, a.n_dims, ns.seed, st, ns.rng_kind,
+                        ns.n_row > 0 ? ns.row_keys : ns.rng_keys, ns.n_row, ns.row_key_stride,
+                        reinterpret_cast<const unsigned long long*>(ns.row_seeds)));
   MSD_CUDA_CHECK(cudaStreamSynchronize(st));
   return 0;
 }

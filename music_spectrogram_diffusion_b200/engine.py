@@ -432,11 +432,14 @@ def op_attention_view(q: torch.Tensor, q_off: int, ldq: int, k: torch.Tensor, k_
       raise ValueError(f'{name}: expected a contiguous f32 tensor of at least {n} elements')
   if not 0 <= splits <= ATTN_MAX_SPLITS or tail < 0 or (acc and tail):
     raise ValueError(f'splits={splits} must be in [0, {ATTN_MAX_SPLITS}]; tail={tail} >= 0 (bf16 only)')
-  lib = _native.load()
-  _native.check(lib.msd_op_attention_view(
-      acc, _ptr(q), q_off, ldq, _ptr(k), k_off, ldk, _ptr(v), v_off, ldv, nb, heads, lq, lk,
-      kv_batch_rows, kv_row0, _ptr(key_mask), mask_len, mask_word0, int(kv_static), _ptr(out), o_col,
-      o_ld, _ptr(part_o), _ptr(part_ml), splits, tail, _stream(q.device)), 'msd_op_attention_view')
+  args = _native.MsdAttentionViewArgs(
+      precision=acc, q=_ptr(q), q_off=q_off, ldq=ldq, k=_ptr(k), k_off=k_off, ldk=ldk, v=_ptr(v), v_off=v_off,
+      ldv=ldv, nb=nb, heads=heads, Lq=lq, Lk=lk, kv_batch_rows=kv_batch_rows, kv_row0=kv_row0,
+      key_mask=_ptr(key_mask), mask_len=mask_len, mask_word0=mask_word0, kv_static=int(kv_static),
+      out=_ptr(out), o_col=o_col, o_ld=o_ld, part_o=_ptr(part_o), part_ml=_ptr(part_ml), splits=splits,
+      tail=tail)
+  _native.check(_native.load().msd_op_attention_view(ctypes.byref(args), _stream(q.device)),
+                'msd_op_attention_view')
 
 
 GEMM_EPILOGUES = dict(EPILOGUES, f32=1, resid_prep=6)
@@ -514,54 +517,56 @@ def op_gemm_view(a: torch.Tensor, a_off: int, lda: int, b: torch.Tensor, b_off: 
       if pos_shift.numel() < -(-m // pos_rows):
         raise ValueError(f'pos_shift: {pos_shift.numel()} entries for {-(-m // pos_rows)} sequences')
   s = _step_value(step, dev)
-  pa = dict(g_lo=None, g_lo_s=0, g_hi=None, g_hi_s=0, split_row=0, a=None, lda=0, ss=None, ss_stride=0)
+  pa = _native.MsdGemmPrep()
   if prep is not None:
     if epilogue != 'resid_prep':
       raise ValueError('prep goes with the resid_prep epilogue')
+    gains = {}
     for key in ('g_lo', 'g_hi'):
       t, off, stride = prep[key]
       if stride and step is None:
         raise ValueError(f'prep.{key}: a step stride needs the device step')
       _check_vector(f'prep.{key}', t, off + s * stride, n, dev)
-      pa[key] = ctypes.c_void_p(t.data_ptr() + 4 * off)
-      pa[key + '_s'] = stride
+      gains[key] = ctypes.c_void_p(t.data_ptr() + 4 * off)
+      gains[key + '_step_stride'] = stride
     _check_dev('prep.a', prep['a'], torch.bfloat16, dev)
     _check_view('prep.a', prep['a'], 0, prep['lda'], m, n, 2)
     _check_dev('prep.ss', prep['ss'], torch.float32, dev)
     if prep['ss_stride'] < m:
       raise ValueError(f'prep.ss_stride {prep["ss_stride"]} < m = {m}')
     _check_view('prep.ss', prep['ss'], 0, prep['ss_stride'], n // (block_n or 64), m, 4)
-    pa.update(split_row=prep['split_row'], a=_ptr(prep['a']), lda=prep['lda'], ss=_ptr(prep['ss']),
-              ss_stride=prep['ss_stride'])
+    pa = _native.MsdGemmPrep(**gains, split_row=prep['split_row'], a=_ptr(prep['a']), lda=prep['lda'],
+                             ss=_ptr(prep['ss']), ss_stride=prep['ss_stride'])
   elif epilogue == 'resid_prep':
     raise ValueError("epilogue 'resid_prep' needs prep")
-  ra = dict(ss_lo=None, parts_lo=0, ss_hi=None, parts_hi=0, split_row=0, ss_stride=0, inv_d=0.0,
-            bias=None, bias_s=0)
+  ra = _native.MsdGemmRowScale()
   if rs is not None:
     if epilogue not in ('bf16', 'gated_gelu'):
       raise ValueError('the row scale goes with the bf16 and gated_gelu epilogues')
+    sums = {}
     for key in ('lo', 'hi'):
       t, parts = rs['ss_' + key], rs['parts_' + key]
       _check_dev(f'rs.ss_{key}', t, torch.float32, dev)
       if parts <= 0 or rs['ss_stride'] < m:
         raise ValueError(f'rs: parts_{key} = {parts} / ss_stride {rs["ss_stride"]} (m = {m})')
       _check_view(f'rs.ss_{key}', t, 0, rs['ss_stride'], parts, m, 4)
-      ra['ss_' + key], ra['parts_' + key] = _ptr(t), parts
-    ra.update(split_row=rs['split_row'], ss_stride=rs['ss_stride'], inv_d=rs['inv_d'])
+      sums['ss_' + key], sums['parts_' + key] = _ptr(t), parts
     if rs.get('bias') is not None:
       t, off, stride = rs['bias']
       if stride and step is None:
         raise ValueError('rs.bias: a step stride needs the device step')
       _check_vector('rs.bias', t, off + s * stride, n, dev)
-      ra['bias'], ra['bias_s'] = ctypes.c_void_p(t.data_ptr() + 4 * off), stride
+      sums['col_bias'], sums['bias_step_stride'] = ctypes.c_void_p(t.data_ptr() + 4 * off), stride
+    ra = _native.MsdGemmRowScale(**sums, split_row=rs['split_row'], ss_stride=rs['ss_stride'],
+                                 inv_d=rs['inv_d'])
+  args = _native.MsdGemmViewArgs(
+      a=_ptr(a), a_off=a_off, lda=lda, b=_ptr(b), b_off=b_off, ldb=ldb, M=m, N=n, K=k,
+      epilogue=GEMM_EPILOGUES[epilogue], block_n=block_n, variant=variant, out=_ptr(out), out_off=out_off,
+      ldo=ldo, resid=_ptr(resid), resid_off=resid_off, pos=_ptr(pos), pos_rows=pos_rows,
+      pos_shift=_ptr(pos_shift), dup_rows=dup_rows, step=_ptr(step), prep=pa, rs=ra)
   bn = ctypes.c_int32(0)
-  _native.check(_native.load().msd_op_gemm_view(
-      _ptr(a), a_off, lda, _ptr(b), b_off, ldb, m, n, k, GEMM_EPILOGUES[epilogue], block_n, variant,
-      _ptr(out), out_off, ldo, _ptr(resid), resid_off, _ptr(pos), pos_rows, _ptr(pos_shift), dup_rows,
-      _ptr(step), pa['g_lo'], pa['g_lo_s'], pa['g_hi'], pa['g_hi_s'], pa['split_row'], pa['a'], pa['lda'],
-      pa['ss'], pa['ss_stride'], ra['ss_lo'], ra['parts_lo'], ra['ss_hi'], ra['parts_hi'],
-      ra['split_row'], ra['ss_stride'], ra['inv_d'], ra['bias'], ra['bias_s'], ctypes.byref(bn),
-      _stream(dev)), 'msd_op_gemm_view')
+  _native.check(_native.load().msd_op_gemm_view(ctypes.byref(args), ctypes.byref(bn), _stream(dev)),
+                'msd_op_gemm_view')
   return bn.value
 
 
@@ -682,13 +687,18 @@ def op_sampler_step(eps: torch.Tensor, z: torch.Tensor, z_split: torch.Tensor, c
     _check_flat('noise', noise, torch.float32, dev, steps * n)
   else:
     _check_streams(n, steps, rng_kind, rng_keys, n_row, row_keys, row_key_stride, row_seeds, per_row, dev)
+  streams = _native.MsdNoiseStreams(
+      seed=int(seed) & 0xFFFFFFFFFFFFFFFF, rng_kind=rng_kind, rng_keys=_ptr(rng_keys), n_row=n_row,
+      row_keys=_ptr(row_keys), row_key_stride=row_key_stride, row_seeds=_ptr(row_seeds))
+  args = _native.MsdSamplerStepArgs(
+      eps=_ptr(eps), z=_ptr(z), z_split=_ptr(z_split), mel_out=_ptr(mel_out), noise=_ptr(noise),
+      coef=_ptr(coef), num_steps=steps, step=_ptr(step), n=n, n_dims=n_dims, passes=passes,
+      cond_weight=float(cond_weight), clip_x0=int(bool(clip_x0)), ddim=int(bool(ddim)),
+      feat_min=float(feat_min), feat_max=float(feat_max), streams=streams,
+      run_step=0 if run_step is None else first, per_row=int(bool(per_row)), launches=launches)
   run_out = (ctypes.c_int32 * 2)()
-  _native.check(_native.load().msd_op_sampler_step(
-      _ptr(eps), _ptr(z), _ptr(z_split), _ptr(mel_out), _ptr(noise), _ptr(coef), steps, _ptr(step), n,
-      n_dims, passes, float(cond_weight), int(bool(clip_x0)), int(bool(ddim)), float(feat_min),
-      float(feat_max), int(seed) & 0xFFFFFFFFFFFFFFFF, rng_kind, _ptr(rng_keys), n_row, _ptr(row_keys),
-      row_key_stride, _ptr(row_seeds), 0 if run_step is None else first, int(bool(per_row)), launches,
-      run_out, _stream(dev)), 'msd_op_sampler_step')
+  _native.check(_native.load().msd_op_sampler_step(ctypes.byref(args), run_out, _stream(dev)),
+                'msd_op_sampler_step')
   return None if run_step is None else (run_out[0], run_out[1])
 
 
@@ -706,9 +716,12 @@ def op_init_z(z: torch.Tensor, z_split: torch.Tensor, n: int, n_dims: int = 128,
     _check_flat('init_z', init_z, torch.float32, dev, n)
   else:
     _check_streams(n, 0, rng_kind, rng_keys, n_row, rng_keys, row_key_stride, row_seeds, n_row > 0, dev)
-  _native.check(_native.load().msd_op_init_z(
-      _ptr(init_z), _ptr(z), _ptr(z_split), n, n_dims, int(seed) & 0xFFFFFFFFFFFFFFFF, rng_kind,
-      _ptr(rng_keys), n_row, row_key_stride, _ptr(row_seeds), _stream(dev)), 'msd_op_init_z')
+  streams = _native.MsdNoiseStreams(
+      seed=int(seed) & 0xFFFFFFFFFFFFFFFF, rng_kind=rng_kind, rng_keys=_ptr(rng_keys), n_row=n_row,
+      row_keys=_ptr(rng_keys), row_key_stride=row_key_stride, row_seeds=_ptr(row_seeds))
+  args = _native.MsdInitZArgs(init_z=_ptr(init_z), z=_ptr(z), z_split=_ptr(z_split), n=n, n_dims=n_dims,
+                              streams=streams)
+  _native.check(_native.load().msd_op_init_z(ctypes.byref(args), _stream(dev)), 'msd_op_init_z')
 
 
 def op_scale_split(feat: torch.Tensor, feat_min: float, feat_max: float,

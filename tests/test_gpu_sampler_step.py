@@ -396,7 +396,7 @@ def test_engine_table_equals_step_table_for(cuda_device):
       eng.close()
 
 
-def test_sampler_step_refuses_bad_arguments(cuda_device):
+def test_sampler_step_refuses_bad_arguments_through_its_struct(cuda_device):
   dev = cuda_device
   tab = torch.from_numpy(table('ddpm', 'large', 'eps')).to(dev)
   n = 1024
@@ -418,8 +418,11 @@ def test_sampler_step_refuses_bad_arguments(cuda_device):
   lib = engine._native.load()
   run_out = (engine.ctypes.c_int32 * 2)()
   for passes, step, per_row, n_row in ((3, 1, 0, 0), (1, STEPS, 0, 0), (1, 1, 1, 12)):
-    rc = lib.msd_op_sampler_step(engine._ptr(eps), engine._ptr(z), engine._ptr(zs), None, None, engine._ptr(tab),
-                                 STEPS, None, n, ND, passes, 1.0, 1, 0, FMIN, FMAX, 0, 0, None, n_row, None, 0,
-                                 None, step, per_row, 1, run_out, None)
+    args = engine._native.MsdSamplerStepArgs(
+        eps=engine._ptr(eps), z=engine._ptr(z), z_split=engine._ptr(zs), coef=engine._ptr(tab), num_steps=STEPS,
+        n=n, n_dims=ND, passes=passes, cond_weight=1.0, clip_x0=1, ddim=0, feat_min=FMIN, feat_max=FMAX,
+        streams=engine._native.MsdNoiseStreams(n_row=n_row), run_step=step, per_row=per_row, launches=1)
+    rc = lib.msd_op_sampler_step(engine.ctypes.byref(args), run_out, None)
     assert rc == -1, (passes, step, per_row)
+  assert lib.msd_op_sampler_step(None, run_out, None) == -1
   assert z.abs().sum().item() == 0

@@ -132,7 +132,7 @@ def test_audio_codec_scaling():
     ac.decode(f)
 
 
-def test_c_abi_exports_every_declared_symbol(native_lib):
+def test_c_abi_7_exports_every_declared_symbol(native_lib):
   """Every function include/msd_b200.h declares is exported, and nothing is bound twice."""
   hdr = open(os.path.join(ROOT, 'include', 'msd_b200.h')).read()
   hdr = re.sub(r'/\*.*?\*/', '', hdr, flags=re.S)
@@ -142,7 +142,7 @@ def test_c_abi_exports_every_declared_symbol(native_lib):
   assert declared == bound, (declared ^ bound)
   for name in declared:
     assert hasattr(native_lib, name), name
-  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 6
+  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 7
   assert isinstance(native_lib.msd_last_error(), bytes)
 
 
@@ -237,7 +237,7 @@ def test_header_is_plain_c(tmp_path):
     pytest.skip('no gcc')
   hdr = os.path.join(ROOT, 'include', 'msd_b200.h')
   for cmd in (['gcc', '-std=c99', '-Wall', '-Wextra', '-pedantic', '-fsyntax-only', '-x', 'c', hdr],
-              ['g++', '-std=c++17', '-fsyntax-only', '-x', 'c++', hdr]):
+              ['g++', '-std=c++17', '-Wall', '-Wextra', '-pedantic', '-fsyntax-only', '-x', 'c++', hdr]):
     r = subprocess.run(cmd, capture_output=True, text=True)
     assert r.returncode == 0 and not r.stderr.strip(), r.stderr
   src = tmp_path / 'layout.c'
@@ -252,6 +252,68 @@ def test_header_is_plain_c(tmp_path):
   assert [int(x) for x in out] == [ctypes.sizeof(_native.MsdConfig), _native.MsdConfig.precision.offset,
                                    ctypes.sizeof(_native.MsdTensor), _native.MsdTensor.shape.offset,
                                    _native.ABI_VERSION]
+
+
+# Every ctypes struct of the binding and the C struct of include/msd_b200.h it mirrors
+C_STRUCTS = {
+    _native.MsdConfig: 'msd_config', _native.MsdTensor: 'msd_tensor',
+    _native.MsdAttentionViewArgs: 'msd_attention_view_args', _native.MsdGemmPrep: 'msd_gemm_prep',
+    _native.MsdGemmRowScale: 'msd_gemm_row_scale', _native.MsdGemmViewArgs: 'msd_gemm_view_args',
+    _native.MsdNoiseStreams: 'msd_noise_streams', _native.MsdSamplerStepArgs: 'msd_sampler_step_args',
+    _native.MsdInitZArgs: 'msd_init_z_args',
+}
+
+
+def _ctypes_fields(cls, prefix=''):
+  """(member path, offset, size) of every field of cls, nested structures field by field."""
+  out = []
+  for name, typ in cls._fields_:
+    f = getattr(cls, name)
+    out.append((prefix + name, f.offset, f.size))
+    if issubclass(typ, ctypes.Structure):
+      out += [(path, f.offset + off, size) for path, off, size in _ctypes_fields(typ, prefix + name + '.')]
+  return out
+
+
+def _header_field_names(hdr: str, cname: str):
+  """The member names of `typedef struct cname { ... } cname;` in declaration order."""
+  body = re.search(r'typedef struct %s \{(.*?)\} %s;' % (cname, cname), hdr, flags=re.S)
+  assert body, cname
+  names = []
+  for decl in body.group(1).split(';')[:-1]:
+    names += [re.search(r'(\w+)\s*(\[\d+\])?\s*$', d).group(1) for d in decl.split(',')]
+  return names
+
+
+def test_ctypes_structs_match_header(tmp_path):
+  """Every ctypes struct of the binding declares the members of its C struct in the same order, and
+  a C compiler gives the struct, and every member (nested ones too), the size and offset ctypes
+  gives it: a field missing, reordered or resized on either side fails here, without a GPU."""
+  import shutil
+  import subprocess
+  if not shutil.which('gcc'):
+    pytest.skip('no gcc')
+  defined = {v for v in vars(_native).values() if isinstance(v, type) and issubclass(v, ctypes.Structure)}
+  assert defined == set(C_STRUCTS)
+  hdr = re.sub(r'/\*.*?\*/', '', open(os.path.join(ROOT, 'include', 'msd_b200.h')).read(), flags=re.S)
+  prints, want = [], []
+  for cls, cname in C_STRUCTS.items():
+    assert _header_field_names(hdr, cname) == [name for name, _ in cls._fields_], cname
+    prints.append(f'printf("{cname} %zu\\n", sizeof({cname}));')
+    want.append(f'{cname} {ctypes.sizeof(cls)}')
+    for path, off, size in _ctypes_fields(cls):
+      prints.append(f'printf("{cname}.{path} %zu %zu\\n", offsetof({cname}, {path}), '
+                    f'sizeof((({cname}*)0)->{path}));')
+      want.append(f'{cname}.{path} {off} {size}')
+  src = tmp_path / 'fields.c'
+  src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "msd_b200.h"\nint main(void) {\n' +
+                 '\n'.join(prints) + '\nreturn 0;\n}\n')
+  exe = tmp_path / 'fields'
+  r = subprocess.run(['gcc', '-std=c99', '-Wall', '-I', os.path.join(ROOT, 'include'), str(src), '-o',
+                      str(exe)], capture_output=True, text=True)
+  assert r.returncode == 0, r.stderr
+  got = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines()
+  assert got == want
 
 
 def test_stale_library_is_refused(monkeypatch, native_lib):
