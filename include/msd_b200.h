@@ -22,7 +22,9 @@
 extern "C" {
 #endif
 
-#define MSD_B200_ABI_VERSION 7
+/* ABI 8: the plain f32 dense hooks are gone (msd_op_dense_epilogue runs epilogue 1), and block_n
+ * alone sets the GEMM tile width (no `variant` in msd_gemm_view_args or msd_bench_gemm). */
+#define MSD_B200_ABI_VERSION 8
 
 typedef struct msd_ctx msd_ctx;
 
@@ -185,21 +187,11 @@ uint64_t msd_launch_count(void);
 
 /* ---- operator-level entry points (unit parity against msd/layers.py) ------------------- */
 
-/* DenseGeneral (layers.py:397-442): out[M,N] f32 = A[M,K] * W, with A given as bf16-rounded
- * f32 [M,K] device and W as f32 [K,N] host-layout device pointer (packed internally). */
-int msd_op_dense(const float* a, const float* w, int32_t M, int32_t N, int32_t K, float* out,
-                 void* stream);
-
-/* Same, selecting the tile-width choice: variant 0 = widest tile that fills the SMs (default),
- * 1 = power-of-two widths only; block_n 0 = auto or one of 64/128/192/256 (192 only with variant 0). */
-int msd_op_dense_variant(const float* a, const float* w, int32_t M, int32_t N, int32_t K,
-                         float* out, int32_t variant, int32_t block_n, void* stream);
-
 /* Micro-benchmark hook: average milliseconds of `iters` back-to-back launches of the bf16 GEMM
- * [M,K] x [N,K]^T with the given epilogue (0 bf16, 1 f32, 2 f32 + residual, 3 gated-GELU) on
- * zero-filled scratch buffers. */
-int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t variant,
-                   int32_t block_n, int32_t iters, float* ms_out);
+ * [M,K] x [N,K]^T with the given epilogue (0 bf16, 1 f32, 2 f32 + residual in place, 3 gated-GELU)
+ * on zero-filled scratch buffers; block_n as in msd_gemm_view_args. */
+int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n, int32_t iters,
+                   float* ms_out);
 
 /* Micro-benchmark hook: average milliseconds of `iters` back-to-back launches of the bf16
  * attention kernel (+ its combine kernel when the keys are split) on scratch
@@ -214,8 +206,10 @@ int msd_bench_attention(int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, int32
 int msd_op_attention(const float* q, const float* k, const float* v, const int32_t* key_mask,
                      int32_t nb, int32_t heads, int32_t Lq, int32_t Lk, float* out, void* stream);
 
-/* DenseGeneral with each fused epilogue of the hot path (kernels.h GemmEpilogue), for unit parity:
+/* DenseGeneral (layers.py:397-442) with each fused epilogue of the hot path (kernels.h
+ * GemmEpilogue), for unit parity:
  *   0 bf16 out                      out [M, N]            = bf16(a w)
+ *   1 f32 out                       out [M, N]            = a w
  *   2 f32 + residual                out [M, N]            = a w + resid [M, N]
  *   3 gated GELU (layers.py:483-509) out [M, N]           = bf16(gelu_tanh(a w) * (a w1)), w / w1 [K, N]
  *   4 f32 + position rows           out [M (+ dup), N]    = a w + pos[(r % pos_rows - shift[r /
@@ -224,8 +218,8 @@ int msd_op_attention(const float* q, const float* k, const float* v, const int32
  *   5 gated GELU, fp32-accurate     out [M, N]            = hi + lo of the [hi | lo | hi] output,
  *                                    computed from 3 x bf16 split operands (a, w, w1 used in full
  *                                    fp32 precision)
- * a [M, K], w [K, N] f32 device (bf16-rounded by the caller for epilogues 0-4); block_n 0 = auto.
- * Unused pointers may be NULL.  out is f32 device. */
+ * a [M, K], w [K, N] f32 device (bf16-rounded by the caller for epilogues 0-4; w is packed
+ * internally); block_n as in msd_gemm_view_args.  Unused pointers may be NULL.  out is f32 device. */
 int msd_op_dense_epilogue(const float* a, const float* w, const float* w1, int32_t M, int32_t N,
                           int32_t K, int32_t epilogue, int32_t block_n, const float* resid,
                           const float* pos, int32_t pos_rows, const int32_t* pos_shift,
@@ -347,8 +341,7 @@ typedef struct msd_gemm_view_args {
                                  position rows, 5 gated GELU split [hi | lo | hi] (bf16 [M, 3 N / 2]),
                                  6 deferred-normalisation producer (out == resid, f32 in place; see
                                  msd_op_dense_deferred_norm) */
-  int32_t block_n;            /* 0 = automatic, else 64 / 96 / 128 / 192 / 256 */
-  int32_t variant;            /* as in msd_op_dense_variant */
+  int32_t block_n;            /* 0 = automatic, else 64 / 96 (fp32 outputs) / 128 / 192 / 256 */
   void* out;                  /* f32 (epilogues 1, 2, 4, 6) or bf16 (0, 3, 5) at element offset
                                  out_off, row stride ldo */
   int64_t out_off;

@@ -148,7 +148,7 @@ class MsdGemmViewArgs(ctypes.Structure):
   __slots__ = ()
   _fields_ = [
       ('a', _P), ('a_off', _L), ('lda', _I), ('b', _P), ('b_off', _L), ('ldb', _I),
-      ('M', _I), ('N', _I), ('K', _I), ('epilogue', _I), ('block_n', _I), ('variant', _I),
+      ('M', _I), ('N', _I), ('K', _I), ('epilogue', _I), ('block_n', _I),
       ('out', _P), ('out_off', _L), ('ldo', _I), ('resid', _P), ('resid_off', _L),
       ('pos', _P), ('pos_rows', _I), ('pos_shift', _P), ('dup_rows', _I), ('step', _P),
       ('prep', MsdGemmPrep), ('rs', MsdGemmRowScale),
@@ -202,9 +202,7 @@ SYMBOLS = [
     ('msd_step_table', ctypes.c_int, [ctypes.POINTER(MsdConfig), _P]),
     ('msd_profile_step', ctypes.c_int, [_P, _I, _I, _P]),
     ('msd_launch_count', ctypes.c_uint64, []),
-    ('msd_op_dense', ctypes.c_int, [_P, _P, _I, _I, _I, _P, _P]),
-    ('msd_op_dense_variant', ctypes.c_int, [_P, _P, _I, _I, _I, _P, _I, _I, _P]),
-    ('msd_bench_gemm', ctypes.c_int, [_I, _I, _I, _I, _I, _I, _I, ctypes.POINTER(ctypes.c_float)]),
+    ('msd_bench_gemm', ctypes.c_int, [_I, _I, _I, _I, _I, _I, ctypes.POINTER(ctypes.c_float)]),
     ('msd_bench_attention', ctypes.c_int, [_I, _I, _I, _I, _I, ctypes.POINTER(ctypes.c_float)]),
     ('msd_op_attention', ctypes.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
     ('msd_op_rmsnorm_film', ctypes.c_int, [_P, _P, _P, _I, _I, _P, _P]),
@@ -232,7 +230,7 @@ SYMBOLS = [
      [_P, _I, ctypes.c_int64, _P, _P, _P, _P, ctypes.c_float, _I, _P]),
     ('msd_op_griffin_lim_istft', ctypes.c_int, [_P, _P, _I, ctypes.c_int64, _P, _P, _P]),
 ]
-ABI_VERSION = 7  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
+ABI_VERSION = 8  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
 
 _lib: Optional[ctypes.CDLL] = None
 

@@ -278,9 +278,7 @@ int launch_attention_f32(const AttnF32Args& a, cudaStream_t stream) {
     if (a.splits > 0) {
       splits = a.splits;
     } else {
-      int sms = 132, dev = 0;
-      if (cudaGetDevice(&dev) == cudaSuccess)
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+      const int sms = device_sm_count();
       for (int s = 2; s <= a.max_splits && ctas * (s - 1) < 3 * sms; ++s)
         if (nkb % s == 0 && nkb / s >= 4) splits = s;
     }

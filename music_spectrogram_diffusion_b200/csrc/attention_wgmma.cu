@@ -321,20 +321,6 @@ attention_combine_kernel(const float* __restrict__ part_o, const float* __restri
 
 }  // namespace
 
-// SMs of the current device (132 on H100 SXM).
-static int device_sm_count() {
-  static thread_local int cached_dev = -1, cached = 132;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  if (dev != cached_dev) {
-    int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    cached = n;
-    cached_dev = dev;
-  }
-  return cached;
-}
-
 // Which instance runs: 128-key blocks unless MSD_ATTN_BKV=64 asks for the small one.
 static int attention_bkv(int Lk) {
   const char* e = getenv("MSD_ATTN_BKV");  // read per launch: the tests switch instances

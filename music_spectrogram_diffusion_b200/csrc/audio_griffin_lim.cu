@@ -319,13 +319,6 @@ gl_tile_kernel(const float* __restrict__ mag, const float2* __restrict__ angles_
   }
 }
 
-int sm_count(int* sms) {
-  int dev = 0;
-  MSD_CUDA_CHECK(cudaGetDevice(&dev));
-  MSD_CUDA_CHECK(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
-}
-
 template <typename Kernel>
 int launch_tiles(Kernel kernel, long long grid, const float* mag, const float2* angles_in,
                  long long frames, const float* window, float coef, float2* angles_out,
@@ -348,14 +341,13 @@ int launch_gl_nnls(const float* features, long long total, const float* weights,
   const int smem = static_cast<int>(sizeof(NnlsSmem));
   MSD_CUDA_CHECK(cudaFuncSetAttribute(gl_nnls_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       smem));
-  int sms = 0, per_sm = 0;
-  if (int rc = sm_count(&sms)) return rc;
+  int per_sm = 0;
   MSD_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gl_nnls_kernel, kThreads,
                                                                smem));
   MSD_REQUIRE(per_sm > 0, "griffin_lim nnls: the kernel does not fit on an SM");
   // one wave of CTAs, each walking frames with a stride: the table set-up is paid once per CTA
   const long long want = (total + kWarps - 1) / kWarps;
-  const long long cap = static_cast<long long>(sms) * per_sm;
+  const long long cap = static_cast<long long>(device_sm_count()) * per_sm;
   gl_nnls_kernel<<<static_cast<unsigned>(want < cap ? want : cap), kThreads, smem, stream>>>(
       features, total, weights, pinv, inv_l, beta, n_iter, mag);
   MSD_CUDA_CHECK(cudaGetLastError());
@@ -369,10 +361,8 @@ int launch_gl_phase_init(int rows, long long frames, unsigned long long seed, fl
   const long long quads = (per_row + 3) / 4;
   const long long total = rows * quads;
   if (total == 0) return 0;
-  int sms = 0;
-  if (int rc = sm_count(&sms)) return rc;
   const long long want = (total + kThreads - 1) / kThreads;
-  const long long cap = static_cast<long long>(sms) * 16;
+  const long long cap = static_cast<long long>(device_sm_count()) * 16;
   gl_phase_init_kernel<<<static_cast<unsigned>(want < cap ? want : cap), kThreads, 0, stream>>>(
       per_row, quads, total, seed, angles);
   MSD_CUDA_CHECK(cudaGetLastError());

@@ -143,9 +143,8 @@ int launch_audio_mel(const float* audio, int rows, long long n_samples, const fl
   const int smem = static_cast<int>(sizeof(MelSmem));
   MSD_CUDA_CHECK(cudaFuncSetAttribute(audio_mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       smem));
-  int dev = 0, sms = 0, per_sm = 0;
-  MSD_CUDA_CHECK(cudaGetDevice(&dev));
-  MSD_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int sms = device_sm_count();
+  int per_sm = 0;
   MSD_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, audio_mel_kernel, kThreads,
                                                                smem));
   MSD_REQUIRE(per_sm > 0, "audio_mel: the kernel does not fit on an SM");

@@ -70,6 +70,19 @@ void prof_begin(int cls, double flops, double bytes, cudaStream_t st) {
 }
 void prof_end(cudaStream_t st) { cudaEventRecord(g_prof->recs.back().e1, st); }
 
+int device_sm_count() {
+  static thread_local int cached_dev = -1, cached = 132;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (dev != cached_dev) {
+    int n = 0;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    cached = n;
+    cached_dev = dev;
+  }
+  return cached;
+}
+
 // ---------------------------------------------------------------------------
 // TMA tensor map encoder (driver entry point resolved through the runtime)
 // ---------------------------------------------------------------------------
@@ -197,9 +210,8 @@ struct msd_ctx {
   int ks = 1;
   bool weights_loaded = false;
   Arena arena;
-  cudaStream_t work = nullptr, work2 = nullptr;
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_fork = nullptr, ev_join = nullptr;
-  bool two_streams = false;
+  cudaStream_t work = nullptr;
+  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
 
   // ---- parameters
   float* tok_emb = nullptr;  // [vocab, d] f32
@@ -769,8 +781,8 @@ static int cross_attention(const msd_ctx* c, int l, int nseg, bf16* o, cudaStrea
 
 // A pre-norm (+FiLM) of a decoder layer (layers.py:632-666) takes one of two forms, and only
 // normed_proj and resid_proj below know which.  Stand-alone: an rmsnorm (+FiLM) kernel writes the
-// normalised operand of the projection.  DEFERRED NORMALISATION (bf16 mode, one chain; kernels.h
-// GemmPrep / GemmRowScale): the norm is split into a column gain applied where the residual stream
+// normalised operand of the projection.  DEFERRED NORMALISATION (bf16 mode; kernels.h GemmPrep /
+// GemmRowScale): the norm is split into a column gain applied where the residual stream
 // is produced and a row scale + bias row applied where the next projection's accumulator is
 // drained,
 //     (rmsnorm(x) gamma (1 + fs) + fb) W  ==  rsqrt(mean(x^2) + eps) * ((x gamma (1 + fs)) W) + fb W,
@@ -793,12 +805,10 @@ struct PreNorm {
   RowSums* hi;         //   that prepares it writes them there), and those it reads for the others
 };
 
-// Rows [seg0 * N, (seg0 + nseg) * N) of the decoder's buffers, of which the first Rc cross-attend
+// The decoder's row buffers, of which the first Rc rows cross-attend
 struct LayerRows {
   msd_ctx* c;
   int Rc;
-  float* x;
-  bf16* xn;
   cudaStream_t st;
 };
 
@@ -823,19 +833,19 @@ static int normed_proj(const LayerRows& s, const PreNorm& p, const bf16* W, int 
   msd_ctx* c = s.c;
   const int d = c->d;
   if (!c->fused_norm) {
-    MSD_TRY(norm_into(c, s.x, p.gamma, M, s.xn, p.film >= 0 ? c->film : nullptr,
+    MSD_TRY(norm_into(c, c->x, p.gamma, M, c->xn, p.film >= 0 ? c->film : nullptr,
                       p.film >= 0 ? static_cast<long long>(p.film) * 2 * d : 0, s.st));
-    return dense(c, s.xn, W, M, N, d, epi, out, ldo, nullptr, s.st);
+    return dense(c, c->xn, W, M, N, d, epi, out, ldo, nullptr, s.st);
   }
   if (p.lo->parts == 0) {
     // no residual epilogue has prepared these rows: layer 0's stream comes from the input projection
     long long gs = 0;
     const float* g = col_gain(c, p, &gs);
-    MSD_TRY(launch_prep_rows(s.x, g, gs, c->d_step, M, d, s.xn, d, p.lo->ss, s.st));
+    MSD_TRY(launch_prep_rows(c->x, g, gs, c->d_step, M, d, c->xn, d, p.lo->ss, s.st));
     p.lo->parts = 1;
   }
   const int Ld = c->cfg.num_decoder_layers;
-  GemmArgs a = deferred_args(c, s.xn, d, W, M, N, d, epi, out, ldo);
+  GemmArgs a = deferred_args(c, c->xn, d, W, M, N, d, epi, out, ldo);
   a.rs.ss_lo = p.lo->ss; a.rs.parts_lo = p.lo->parts;
   a.rs.ss_hi = p.hi->ss; a.rs.parts_hi = p.hi->parts;
   a.rs.split_row = p.lo == p.hi ? M : s.Rc;   // one buffer serves all M rows
@@ -854,13 +864,13 @@ static int resid_proj(const LayerRows& s, const bf16* A, const bf16* W, int M, i
                       const PreNorm* hi, int split) {
   msd_ctx* c = s.c;
   const int d = c->d;
-  if (!c->fused_norm || lo == nullptr) return dense(c, A, W, M, d, K, EPI_RESID_F32, s.x, d, s.x, s.st);
-  GemmArgs a = deferred_args(c, A, K, W, M, d, K, EPI_RESID_PREP, s.x, d);
-  a.resid = s.x;
+  if (!c->fused_norm || lo == nullptr) return dense(c, A, W, M, d, K, EPI_RESID_F32, c->x, d, c->x, s.st);
+  GemmArgs a = deferred_args(c, A, K, W, M, d, K, EPI_RESID_PREP, c->x, d);
+  a.resid = c->x;
   a.prep.g_lo = col_gain(c, *lo, &a.prep.g_lo_step_stride);
   a.prep.g_hi = col_gain(c, *hi, &a.prep.g_hi_step_stride);
   a.prep.split_row = split;
-  a.prep.a = s.xn; a.prep.lda = d;
+  a.prep.a = c->xn; a.prep.lda = d;
   a.prep.ss = lo->lo->ss; a.prep.ss_stride = c->passes * c->Bmax * c->N;
   const int bn = gemm_resolve_block_n(a);   // the partial row sums are per column tile that runs
   MSD_REQUIRE(bn > 0, "resid_proj: no tile width for M=%d d=%d", M, d);
@@ -868,22 +878,17 @@ static int resid_proj(const LayerRows& s, const bf16* A, const bf16* W, int M, i
   return launch_gemm(a, s.st);
 }
 
-// The 12 DecoderLayers (network.py:161-258) over segments [seg0, seg0 + nseg) of the row buffers.
+// The 12 DecoderLayers (network.py:161-258) over the first `nseg` segments of the row buffers.
 // The first `ncross` of these segments cross-attend to the cached encodings (conditional pass;
 // the unconditional rows skip the block: with encodings and masks multiplied by 0 it is exactly
 // 0); every other kernel batches all rows.
-static int decoder_layers(msd_ctx* c, int seg0, int nseg, int ncross, cudaStream_t st) {
-  const int d = c->d, hh = c->hh, F = c->F, N = c->N, ks = c->ks;
+static int decoder_layers(msd_ctx* c, int nseg, int ncross, cudaStream_t st) {
+  const int hh = c->hh, F = c->F, N = c->N, ks = c->ks;
   const int R = nseg * N, Rc = ncross * N;
   const int Ld = c->cfg.num_decoder_layers;
   const int nsrc = c->nsrc;
-  const size_t r0 = static_cast<size_t>(seg0) * N;
-  // views of the row buffers (disjoint per range); a GEMM-input row is ks x wider
-  const LayerRows s = {c, Rc, c->x + r0 * d, c->xn + r0 * d * ks, st};
-  const size_t qkv_off = r0 * 3 * hh;
-  bf16* attn = c->attn + r0 * hh * ks;
-  bf16* hmid = c->hmid + r0 * F * ks;
-  bf16* cross_o = nsrc == 1 ? attn : c->attn2;
+  const LayerRows s = {c, Rc, st};
+  bf16* cross_o = nsrc == 1 ? c->attn : c->attn2;
   RowSums sx = {c->ss_x, 0}, so = {c->ss_so, 0}, co = {c->ss_co, 0};
   auto self_norm = [&](int l) {
     return PreNorm{c->dec[l].ln_self, 2 * l, c->btab_qkv, 3 * hh, l, &sx, &sx};
@@ -895,11 +900,11 @@ static int decoder_layers(msd_ctx* c, int seg0, int nseg, int ncross, cudaStream
     // rows that skip the cross-attention keep the row sums of the self-attention projection
     const PreNorm mlp = {w.ln_mlp, 2 * l + 1, c->btab_wi, 2 * F, l, Rc > 0 ? &co : &so, &so};
     // self-attention block (174-193)
-    MSD_TRY(normed_proj(s, self, w.self_attn.qkv, R, 3 * hh, epi_qkv(c), at(c, c->qkv, qkv_off), 3 * hh));
-    MSD_TRY(attention(c, c->qkv, qkv_off, 3 * hh, c->qkv, qkv_off + hh, 3 * hh, c->qkv,
-                      qkv_off + 2 * hh, 3 * hh, attn, hh, 0, nseg, c->H, N, N, nullptr, 0, st));
+    MSD_TRY(normed_proj(s, self, w.self_attn.qkv, R, 3 * hh, epi_qkv(c), c->qkv, 3 * hh));
+    MSD_TRY(attention(c, c->qkv, 0, 3 * hh, c->qkv, hh, 3 * hh, c->qkv, 2 * hh, 3 * hh, c->attn, hh, 0, nseg,
+                      c->H, N, N, nullptr, 0, st));
     // rows that cross-attend are prepared for the cross-attention's pre-norm, the others for the MLP's
-    MSD_TRY(resid_proj(s, attn, w.self_attn.out, R, hh, Rc > 0 ? &cross : &mlp, &mlp, Rc));
+    MSD_TRY(resid_proj(s, c->attn, w.self_attn.out, R, hh, Rc > 0 ? &cross : &mlp, &mlp, Rc));
     // cross-attention block (196-235), conditioned rows only
     if (Rc > 0) {
       MSD_TRY(normed_proj(s, cross, w.cross_q, Rc, nsrc * hh, epi_qkv(c), c->qc, nsrc * hh));
@@ -907,12 +912,12 @@ static int decoder_layers(msd_ctx* c, int seg0, int nseg, int ncross, cudaStream
       MSD_TRY(resid_proj(s, cross_o, w.cross_out, Rc, nsrc * hh, &mlp, &mlp, Rc));
     }
     // MLP block (241-256)
-    MSD_TRY(normed_proj(s, mlp, w.mlp.wi, R, 2 * F, epi_gated(c), hmid, F * ks));
+    MSD_TRY(normed_proj(s, mlp, w.mlp.wi, R, 2 * F, epi_gated(c), c->hmid, F * ks));
     if (l + 1 < Ld) {
       const PreNorm next = self_norm(l + 1);
-      MSD_TRY(resid_proj(s, hmid, w.mlp.wo, R, F, &next, &next, R));
+      MSD_TRY(resid_proj(s, c->hmid, w.mlp.wo, R, F, &next, &next, R));
     } else {
-      MSD_TRY(resid_proj(s, hmid, w.mlp.wo, R, F, nullptr, nullptr, R));
+      MSD_TRY(resid_proj(s, c->hmid, w.mlp.wo, R, F, nullptr, nullptr, R));
     }
   }
   return 0;
@@ -920,11 +925,7 @@ static int decoder_layers(msd_ctx* c, int seg0, int nseg, int ncross, cudaStream
 
 // Decoder.__call__ (network.py:360-457) over `total` segments of which the first `ncond`
 // cross-attend to the cached encodings.  Input: c->z_split; output: c->eps [total*N, nd].
-// With `two_streams` the conditional and unconditional passes -- independent until the guidance
-// combine -- run as two concurrent kernel chains (fork/join on c->work2); a measured-slower
-// experiment (MSD_TWO_STREAMS=1), see msd_create.
-static int run_decoder(msd_ctx* c, int B, int ncond, int total, cudaStream_t st,
-                       bool two_streams = false) {
+static int run_decoder(msd_ctx* c, int B, int ncond, int total, cudaStream_t st) {
   const int d = c->d, N = c->N, nd = c->nd;
   const int R = total * N;
   // continuous_inputs_projection + position encodings (420-427); both passes start equal.
@@ -934,20 +935,8 @@ static int run_decoder(msd_ctx* c, int B, int ncond, int total, cudaStream_t st,
   g_pdl_skip_next = true;
   MSD_TRY(gemm_pos(c->z_split, 3 * nd, c->dec_in_proj, 3 * nd, B * N, d, 3 * nd, c->x, c->dec_pos,
                    N, nullptr, total > B ? B * N : 0, st));
-  const int nuncond = total - ncond;
-  if (two_streams && ncond > 0 && nuncond > 0) {
-    MSD_CUDA_CHECK(cudaEventRecord(c->ev_fork, st));
-    MSD_CUDA_CHECK(cudaStreamWaitEvent(c->work2, c->ev_fork, 0));
-    g_pdl_skip_next = true;  // first kernel of the side chain depends on another stream
-    MSD_TRY(decoder_layers(c, ncond, nuncond, 0, c->work2));
-    MSD_TRY(decoder_layers(c, 0, ncond, ncond, st));
-    MSD_CUDA_CHECK(cudaEventRecord(c->ev_join, c->work2));
-    MSD_CUDA_CHECK(cudaStreamWaitEvent(st, c->ev_join, 0));
-    g_pdl_skip_next = true;  // the join kernel has two predecessors
-  } else {
-    // one chain, both passes batched per kernel except the cross-attention block
-    MSD_TRY(decoder_layers(c, 0, total, ncond, st));
-  }
+  // both passes batched per kernel except the cross-attention block
+  MSD_TRY(decoder_layers(c, total, ncond, st));
   // decoder_norm + spec_out_dense in split precision (445-456: fp32 "for stability")
   MSD_TRY(launch_rmsnorm(c->x, c->dec_norm, R, d, c->xn, 3 * d, nullptr, nullptr, 0, 0, 1, st));
   MSD_TRY(gemm(c->xn, 3 * d, c->spec_out, 3 * d, R, nd, 3 * d, EPI_F32, c->eps, nd, nullptr, st));
@@ -1069,17 +1058,7 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   const size_t R = static_cast<size_t>(c->passes) * c->Bmax * c->N;
   const size_t BN = static_cast<size_t>(c->Bmax) * c->N;
   const size_t ER = static_cast<size_t>(c->Bmax) * (c->T > c->C ? c->T : c->C);
-  {
-    // Opt-in experiment (MSD_TWO_STREAMS=1): conditional / unconditional passes as two concurrent
-    // kernel chains.  Every GEMM / attention CTA owns a whole SM's shared memory, so the chains
-    // mostly time-share SMs, and the half-height GEMMs are less efficient -> off by default.
-    const char* ts = getenv("MSD_TWO_STREAMS");
-    c->two_streams = (ts && ts[0] == '1') && !c->acc;
-  }
   MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&c->work, cudaStreamNonBlocking));
-  MSD_CUDA_CHECK(cudaStreamCreateWithFlags(&c->work2, cudaStreamNonBlocking));
-  MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
-  MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming));
   MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_in, cudaEventDisableTiming));
   MSD_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_out, cudaEventDisableTiming));
   MSD_TRY(A.alloc(&c->x, R * c->d));
@@ -1100,7 +1079,7 @@ int msd_create(const msd_config* cfg, int device, msd_ctx** out) {
   {
     // MSD_FUSED_NORM=0: tuning / test hook, keeps the stand-alone rmsnorm kernels
     const char* fn = getenv("MSD_FUSED_NORM");
-    c->fused_norm = !c->acc && !c->two_streams && !(fn && fn[0] == '0');
+    c->fused_norm = !c->acc && !(fn && fn[0] == '0');
     if (c->fused_norm) {
       MSD_TRY(A.alloc(&c->ss_x, kSsParts * R));
       MSD_TRY(A.alloc(&c->ss_so, kSsParts * R));
@@ -1151,9 +1130,6 @@ void msd_destroy(msd_ctx* c) {
   c->arena.release();
   if (c->ev_in) cudaEventDestroy(c->ev_in);
   if (c->ev_out) cudaEventDestroy(c->ev_out);
-  if (c->ev_fork) cudaEventDestroy(c->ev_fork);
-  if (c->ev_join) cudaEventDestroy(c->ev_join);
-  if (c->work2) cudaStreamDestroy(c->work2);
   if (c->work) cudaStreamDestroy(c->work);
   delete c;
 }
@@ -1315,8 +1291,8 @@ static int run_steps(msd_ctx* c, const float* noise, unsigned long long seed, in
     const unsigned long long before = g_launch_count;
     cudaGraph_t graph = nullptr;
     MSD_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = c->xrole == 0 ? run_decoder(c, B, B, c->passes * B, st, c->two_streams)
-                           : run_decoder(c, B, c->xrole == 1 ? B : 0, B, st, false);
+    int rc = c->xrole == 0 ? run_decoder(c, B, B, c->passes * B, st)
+                           : run_decoder(c, B, c->xrole == 1 ? B : 0, B, st);
     if (rc == 0) rc = sampler_step(c, B, nullptr, 0, nullptr, st, true);
     cudaError_t ce = cudaStreamEndCapture(st, &graph);
     if (rc != 0) {

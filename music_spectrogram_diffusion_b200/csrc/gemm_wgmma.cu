@@ -18,8 +18,6 @@
 //
 // Replaces the XLA dot_general lowering of DenseGeneral (msd/layers.py:397-442) for every
 // projection on the hot path (SURVEY §2.2 K2, K4, K5, K6, K8, K9).
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "kernels.h"
 #include "wgmma.cuh"
@@ -456,27 +454,13 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
   }
 }
 
-// SMs of the current device (132 on H100 SXM): one CTA is resident per SM.
-static int gemm_sm_count() {
-  static thread_local int cached_dev = -1, cached = 0;
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-  if (dev != cached_dev) {
-    int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-    cached = n;
-    cached_dev = dev;
-  }
-  return cached;
-}
-
 template <int BN>
 int launch_bn(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmDev& d,
               cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
   static_assert(Cfg::SMEM_BYTES <= 227 * 1024 && Cfg::STAGES >= 3, "smem budget");
   const int tiles = (d.N / BN) * (d.M / BLOCK_M);
-  const int sms = gemm_sm_count();
+  const int sms = device_sm_count();  // one CTA is resident per SM
   dim3 grid(tiles < sms ? tiles : sms);
   ProfScope prof(KC_GEMM, 2.0 * d.M * d.N * d.K,
                  2.0 * (static_cast<double>(d.M) * d.K + static_cast<double>(d.N) * d.K) +
@@ -505,15 +489,15 @@ int gemm_configure() {
   return configure_bn<256>();
 }
 
-// Tile width of the default variant.  The CTAs are persistent, one per SM, so a launch takes
-// ceil(tiles / SMs) tile times, and a tile's k-block costs about 4 (BN + 64) cycles (measured 515 /
-// 690 / 983 / 1168 at BN 64 / 128 / 192 / 256): take the width with the least
+// The tile width launch_gemm runs with when block_n is 0.  The CTAs are persistent, one per SM, so
+// a launch takes ceil(tiles / SMs) tile times, and a tile's k-block costs about 4 (BN + 64) cycles
+// (measured 515 / 690 / 983 / 1168 at BN 64 / 128 / 192 / 256): take the width with the least
 // ceil(tiles / SMs) * (BN + 64), the wider one on a tie (it re-reads the least of A and B per FLOP).
 // 96 only for the fp32-output epilogues.
-int gemm_pick_wide_bn(int M, int N, int epilogue) {
+static int gemm_pick_wide_bn(int M, int N, int epilogue) {
   const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
   const int widths[5] = {256, 192, 128, 96, 64};
-  const int sms = gemm_sm_count();
+  const int sms = device_sm_count();
   int best = 0;
   long long best_cost = 0;
   for (int i = 0; i < 5; ++i) {
@@ -526,31 +510,10 @@ int gemm_pick_wide_bn(int M, int N, int epilogue) {
   return best;
 }
 
-// Tile width of variant 1: power-of-two widths only, a wider tile once it fills every SM.
-int gemm_pick_block_n(int M, int N) {
-  const int mt = (M + BLOCK_M - 1) / BLOCK_M;
-  const int sms = gemm_sm_count();
-  if (N % 256 == 0 && mt * (N / 256) >= 2 * sms) return 256;
-  if (N % 128 == 0 && mt * (N / 128) >= sms) return 128;
-  if (N % 64 == 0) return 64;
-  if (N % 128 == 0) return 128;
-  return 0;
-}
-
-static bool gemm_wide_variant(const GemmArgs& a) {
-  static const int forced_variant = [] {
-    const char* e = getenv("MSD_GEMM_VARIANT");  // debugging aid: 1 forces variant 1's tile choice
-    return e ? atoi(e) : 0;
-  }();
-  return (forced_variant ? forced_variant : a.variant) != 1;
-}
-
 int gemm_resolve_block_n(const GemmArgs& a) {
-  const bool wide = gemm_wide_variant(a);
-  const int bn = a.block_n ? a.block_n
-                           : (wide ? gemm_pick_wide_bn(a.M, a.N, a.epilogue) : gemm_pick_block_n(a.M, a.N));
-  const bool allowed = bn == 64 || bn == 128 || bn == 256 || (wide && bn == 192) ||
-                       (wide && bn == 96 && !epi_is_bf16_out(a.epilogue));
+  const int bn = a.block_n ? a.block_n : gemm_pick_wide_bn(a.M, a.N, a.epilogue);
+  const bool allowed = bn == 64 || bn == 128 || bn == 192 || bn == 256 ||
+                       (bn == 96 && !epi_is_bf16_out(a.epilogue));
   return allowed && a.N % bn == 0 ? bn : 0;
 }
 
@@ -561,8 +524,7 @@ int launch_gemm(const GemmArgs& a, cudaStream_t stream) {
   MSD_REQUIRE(a.K % BLOCK_K == 0, "gemm: K=%d must be a multiple of %d", a.K, BLOCK_K);
   MSD_REQUIRE(a.M % BLOCK_M == 0, "gemm: M=%d must be a multiple of %d", a.M, BLOCK_M);
   const int bn = gemm_resolve_block_n(a);
-  MSD_REQUIRE(bn != 0, "gemm: N=%d has no valid tile width (block_n %d, variant %d)", a.N, a.block_n,
-              gemm_wide_variant(a) ? 0 : 1);
+  MSD_REQUIRE(bn != 0, "gemm: N=%d has no valid tile width (block_n %d)", a.N, a.block_n);
   MSD_REQUIRE(a.ldo % 8 == 0, "gemm: ldo=%d must be a multiple of 8", a.ldo);
 
   CUtensorMap ta, tb;

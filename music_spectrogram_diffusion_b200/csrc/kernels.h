@@ -42,7 +42,7 @@ struct ProfScope {
 // PDL is enabled (default; MSD_PDL=0 disables).  Works under stream capture (programmatic edges).
 // ---------------------------------------------------------------------------
 extern bool g_use_pdl;
-extern thread_local bool g_pdl_skip_next;  // next launch (of this host thread) has a cross-stream dependency: plain launch
+extern thread_local bool g_pdl_skip_next;  // next launch (of this host thread) waits for its predecessor to complete: plain launch
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
                                  cudaStream_t stream, Args&&... args) {
@@ -59,6 +59,11 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
   g_pdl_skip_next = false;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
+
+// SMs of the current device (132 on H100 SXM), kept per host thread until it switches devices:
+// every tile, split and grid policy sizes its launches from it.  132 when the device cannot be
+// queried; the launch that follows then reports the CUDA error.
+int device_sm_count();
 
 // ---------------------------------------------------------------------------
 // TMA tensor maps (driver entry point fetched at run time; no libcuda link).
@@ -129,8 +134,6 @@ struct GemmArgs {
   const int* pos_shift;  // EPI_POS_F32: per (r / pos_rows) roll amount or nullptr
   int dup_rows;          // EPI_POS_F32: also store to row r + dup_rows when > 0
   int block_n;           // 0 = auto
-  int variant;           // tile-width choice: 0 = fewest waves of tiles (default, 96 / 192 allowed),
-                         // 1 = power-of-two widths only
   long long* trace;      // debugging: per-tile stamps (8 int64 per tile, first 512 tiles), or null
   // deferred normalisation: prep.a != null with EPI_RESID_PREP; rs.ss_lo != null
   // with EPI_BF16 / EPI_GATED_GELU; `step` is the device step index the strides multiply
@@ -140,12 +143,10 @@ struct GemmArgs {
 };
 int launch_gemm(const GemmArgs& a, cudaStream_t stream);
 int gemm_configure();  // opt in to the kernels' dynamic shared memory sizes (idempotent)
-// Box rows the A / B maps must be built with for a given block_n choice.
-int gemm_pick_block_n(int M, int N);
-int gemm_pick_wide_bn(int M, int N, int epilogue);
-// The tile width launch_gemm(a) runs with (a.block_n, a.variant, MSD_GEMM_VARIANT and the shape),
-// or 0 when that width is not allowed.  Whoever sizes per-tile outputs (EPI_RESID_PREP's partial
-// row sums: N / width of them) must take the width from here.
+// The tile width launch_gemm(a) runs with: a.block_n when given, else the one that takes the
+// fewest tile times on this device's SMs; 0 when that width is not allowed (64 / 128 / 192 / 256,
+// and 96 for the fp32-output epilogues) or does not divide N.  Whoever sizes per-tile outputs
+// (EPI_RESID_PREP's partial row sums: N / width of them) must take the width from here.
 int gemm_resolve_block_n(const GemmArgs& a);
 
 // ---------------------------------------------------------------------------

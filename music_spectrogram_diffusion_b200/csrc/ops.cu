@@ -43,7 +43,7 @@ int launch_attention_view(const AttnView& v, cudaStream_t st) {
 }
 
 // out [M, N] f32 = the GEMM of a [M, K] f32 with w [K, N] f32 (gated epilogues: w and w1, each
-// [K, N]), run with g's epilogue and its operands, tile width and variant.  a is converted and the
+// [K, N]), run with g's epilogue, its operands and its tile width.  a is converted and the
 // weights packed as the engine packs them (EPI_GATED_GELU_SPLIT3: both in split precision); a bf16
 // output is converted back.
 static int dense_f32(const float* a, const float* w, const float* w1, int M, int N, int K, GemmArgs g,
@@ -132,39 +132,24 @@ using namespace msd;
 
 extern "C" {
 
-int msd_op_dense(const float* a, const float* w, int32_t M, int32_t N, int32_t K, float* out,
-                 void* stream) {
-  return msd_op_dense_variant(a, w, M, N, K, out, 0, 0, stream);
-}
-
-int msd_op_dense_variant(const float* a, const float* w, int32_t M, int32_t N, int32_t K,
-                         float* out, int32_t variant, int32_t block_n, void* stream) {
-  MSD_REQUIRE(a && w && out, "msd_op_dense: null argument");
-  GemmArgs g;
-  memset(&g, 0, sizeof(g));
-  g.epilogue = EPI_F32; g.variant = variant; g.block_n = block_n;
-  return dense_f32(a, w, nullptr, M, N, K, g, out, reinterpret_cast<cudaStream_t>(stream));
-}
-
-int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t variant,
-                   int32_t block_n, int32_t iters, float* ms_out) {
+int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t block_n, int32_t iters,
+                   float* ms_out) {
   MSD_REQUIRE(ms_out && iters > 0, "msd_bench_gemm: bad argument");
   TempBufs tb;
   bf16 *a = nullptr, *b = nullptr;
-  float *o = nullptr, *r = nullptr;
+  float* o = nullptr;
   MSD_TRY(tb.get(&a, static_cast<size_t>(M) * K));
   MSD_TRY(tb.get(&b, static_cast<size_t>(N) * K));
   MSD_TRY(tb.get(&o, static_cast<size_t>(M) * N));
-  MSD_TRY(tb.get(&r, static_cast<size_t>(M) * N));
   MSD_CUDA_CHECK(cudaMemset(a, 0, static_cast<size_t>(M) * K * 2));
   MSD_CUDA_CHECK(cudaMemset(b, 0, static_cast<size_t>(N) * K * 2));
-  MSD_CUDA_CHECK(cudaMemset(r, 0, static_cast<size_t>(M) * N * 4));
+  MSD_CUDA_CHECK(cudaMemset(o, 0, static_cast<size_t>(M) * N * 4));
   GemmArgs ga;
   memset(&ga, 0, sizeof(ga));
   ga.A = a; ga.B = b; ga.M = M; ga.N = N; ga.K = K; ga.lda = K; ga.ldb = K;
   ga.epilogue = epilogue; ga.out = o; ga.ldo = (epilogue == EPI_GATED_GELU) ? N / 2 : N;
-  ga.resid = (variant == 1) ? r : o;  // default variant: in place, like the engine
-  ga.variant = variant; ga.block_n = block_n;
+  ga.resid = o;  // in place, like the engine
+  ga.block_n = block_n;
   const bool trace = getenv("MSD_GEMM_TRACE") != nullptr;
   if (trace && (epilogue == EPI_BF16 || epilogue == EPI_GATED_GELU)) {
     // traced like the decoder's QKV / cross-q / wi launches: a row scale from one partial sum per
@@ -182,7 +167,7 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
   MSD_TRY(bs.create());
   const cudaStream_t st = bs.st;
   MSD_TRY(bs.time(iters, [&] { return launch_gemm(ga, st); }, ms_out));
-  if (!trace || variant == 1) return 0;
+  if (!trace) return 0;
   // one more launch with per-tile stamps (after a warm one right before it, like in the loop)
   long long* tr = nullptr;
   MSD_TRY(tb.get(&tr, 8 * 512));
@@ -213,9 +198,11 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
     ++n;
   }
   const double inv_n = n ? 1.0 / n : 0.0;
+  GemmArgs automatic = ga;
+  automatic.block_n = 0;
   fprintf(stderr, "[gemm trace] M=%d N=%d K=%d epi=%d block_n=%d (automatic %d): %d tiles, first start -> "
           "last end %.2f us, mean cycles per tile %.0f: set-up %.0f, main loop %.0f (%.0f per k-block), "
-          "epilogue %.0f\n", M, N, K, epilogue, gemm_resolve_block_n(ga), gemm_pick_wide_bn(M, N, epilogue), n,
+          "epilogue %.0f\n", M, N, K, epilogue, gemm_resolve_block_n(ga), gemm_resolve_block_n(automatic), n,
           (t1 - t0) * 1e-3, sum[0] * inv_n, sum[1] * inv_n, sum[2] * inv_n, sum[2] * inv_n / (K / 64),
           sum[3] * inv_n);
   for (int b = 0; b < 4 && b < 512; ++b) {
@@ -227,9 +214,7 @@ int msd_bench_gemm(int32_t M, int32_t N, int32_t K, int32_t epilogue, int32_t va
   }
   // the tiles of CTA 0 in order: main loop, drain (bf16 outputs: until the last sub-tile is
   // handed to TMA, whose global writes then run under the next tile's main loop)
-  int sms = 0;
-  MSD_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
-  const int grid = std::min(n, sms > 0 ? sms : n);
+  const int grid = std::min(n, device_sm_count());
   for (int b = 0, i = 0; grid > 0 && b < 512; b += grid, ++i) {
     const long long* r = &h[b * 8];
     if (r[1] == 0) break;
@@ -415,7 +400,8 @@ int msd_op_dense_epilogue(const float* a, const float* w, const float* w1, int32
                           int32_t dup_rows, float* out, void* stream) {
   MSD_REQUIRE(a && w && out, "msd_op_dense_epilogue: null argument");
   const bool gated = epilogue == EPI_GATED_GELU || epilogue == EPI_GATED_GELU_SPLIT3;
-  MSD_REQUIRE(epilogue == EPI_BF16 || epilogue == EPI_RESID_F32 || epilogue == EPI_POS_F32 || gated,
+  MSD_REQUIRE(epilogue == EPI_BF16 || epilogue == EPI_F32 || epilogue == EPI_RESID_F32 || epilogue == EPI_POS_F32 ||
+                  gated,
               "msd_op_dense_epilogue: unknown epilogue %d", epilogue);
   MSD_REQUIRE(!gated || w1 != nullptr, "msd_op_dense_epilogue: the gated epilogues need w1");
   MSD_REQUIRE(epilogue != EPI_RESID_F32 || resid != nullptr, "msd_op_dense_epilogue: resid is null");
@@ -579,7 +565,7 @@ int msd_op_gemm_view(const msd_gemm_view_args* args, int32_t* block_n_out, void*
   memset(&g, 0, sizeof(g));
   g.A = static_cast<const bf16*>(v.a) + v.a_off; g.lda = v.lda;
   g.B = static_cast<const bf16*>(v.b) + v.b_off; g.ldb = v.ldb;
-  g.M = v.M; g.N = v.N; g.K = v.K; g.epilogue = v.epilogue; g.block_n = v.block_n; g.variant = v.variant;
+  g.M = v.M; g.N = v.N; g.K = v.K; g.epilogue = v.epilogue; g.block_n = v.block_n;
   g.out = f32_out ? static_cast<void*>(static_cast<float*>(v.out) + v.out_off)
                   : static_cast<void*>(static_cast<bf16*>(v.out) + v.out_off);
   g.ldo = v.ldo;
@@ -599,8 +585,7 @@ int msd_op_gemm_view(const msd_gemm_view_args* args, int32_t* block_n_out, void*
   MSD_REQUIRE(v.epilogue != EPI_POS_F32 || (v.pos != nullptr && v.pos_rows > 0),
               "msd_op_gemm_view: EPI_POS_F32 needs pos / pos_rows");
   const int bn = gemm_resolve_block_n(g);
-  MSD_REQUIRE(bn > 0, "msd_op_gemm_view: N=%d has no tile width (block_n %d, variant %d)", v.N, v.block_n,
-              v.variant);
+  MSD_REQUIRE(bn > 0, "msd_op_gemm_view: N=%d has no tile width (block_n %d)", v.N, v.block_n);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   g_pdl_skip_next = true;   // the operands were just written by the caller's own kernels
   MSD_TRY(launch_gemm(g, st));

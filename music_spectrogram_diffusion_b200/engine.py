@@ -266,17 +266,6 @@ def launch_count() -> int:
 
 
 # ---- operator-level hooks (unit parity with msd/layers.py) --------------------
-def op_dense(a: torch.Tensor, w: torch.Tensor, variant: int = 0, block_n: int = 0) -> torch.Tensor:
-  lib = _native.load()
-  m, k = a.shape
-  n = w.shape[1]
-  out = torch.empty(m, n, dtype=torch.float32, device=a.device)
-  _native.check(lib.msd_op_dense_variant(_ptr(a.contiguous()), _ptr(w.contiguous()), m, n, k,
-                                         _ptr(out), variant, block_n, _stream(a.device)),
-                'msd_op_dense_variant')
-  return out
-
-
 def op_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor,
                  key_mask: Optional[torch.Tensor], heads: int) -> torch.Tensor:
   lib = _native.load()
@@ -299,7 +288,7 @@ def op_rmsnorm_film(x: torch.Tensor, gamma: torch.Tensor,
   return out
 
 
-EPILOGUES = {'bf16': 0, 'resid_f32': 2, 'gated_gelu': 3, 'pos_f32': 4, 'gated_gelu_split3': 5}
+EPILOGUES = {'bf16': 0, 'f32': 1, 'resid_f32': 2, 'gated_gelu': 3, 'pos_f32': 4, 'gated_gelu_split3': 5}
 
 
 def op_dense_epilogue(a: torch.Tensor, w: torch.Tensor, epilogue: str, block_n: int = 0,
@@ -442,7 +431,7 @@ def op_attention_view(q: torch.Tensor, q_off: int, ldq: int, k: torch.Tensor, k_
                 'msd_op_attention_view')
 
 
-GEMM_EPILOGUES = dict(EPILOGUES, f32=1, resid_prep=6)
+GEMM_EPILOGUES = dict(EPILOGUES, resid_prep=6)
 _F32_OUT = ('f32', 'resid_f32', 'pos_f32', 'resid_prep')
 
 
@@ -472,7 +461,7 @@ def _step_value(step: Optional[torch.Tensor], device: torch.device) -> int:
 
 def op_gemm_view(a: torch.Tensor, a_off: int, lda: int, b: torch.Tensor, b_off: int, ldb: int,
                  m: int, n: int, k: int, epilogue: str, out: torch.Tensor, out_off: int, ldo: int,
-                 block_n: int = 0, variant: int = 0, resid: Optional[torch.Tensor] = None,
+                 block_n: int = 0, resid: Optional[torch.Tensor] = None,
                  resid_off: int = 0, pos: Optional[torch.Tensor] = None,
                  pos_shift: Optional[torch.Tensor] = None, dup_rows: int = 0,
                  step: Optional[torch.Tensor] = None, prep: Optional[dict] = None,
@@ -561,7 +550,7 @@ def op_gemm_view(a: torch.Tensor, a_off: int, lda: int, b: torch.Tensor, b_off: 
                                  inv_d=rs['inv_d'])
   args = _native.MsdGemmViewArgs(
       a=_ptr(a), a_off=a_off, lda=lda, b=_ptr(b), b_off=b_off, ldb=ldb, M=m, N=n, K=k,
-      epilogue=GEMM_EPILOGUES[epilogue], block_n=block_n, variant=variant, out=_ptr(out), out_off=out_off,
+      epilogue=GEMM_EPILOGUES[epilogue], block_n=block_n, out=_ptr(out), out_off=out_off,
       ldo=ldo, resid=_ptr(resid), resid_off=resid_off, pos=_ptr(pos), pos_rows=pos_rows,
       pos_shift=_ptr(pos_shift), dup_rows=dup_rows, step=_ptr(step), prep=pa, rs=ra)
   bn = ctypes.c_int32(0)

@@ -1,4 +1,4 @@
-"""-m gpu: the tile width the GEMM picks on its own (block_n 0, default variant), as
+"""-m gpu: the tile width the GEMM picks on its own (block_n 0), as
 msd_op_gemm_view reports it.  The CTAs are persistent, one per SM, so a launch takes
 ceil(tiles / SMs) tile times and a tile costs about BN + 64 column-units: the width with the least
 ceil(tiles / SMs) * (BN + 64) runs, the wider one on a tie, and 96 only when the output is fp32.

@@ -291,52 +291,29 @@ def test_deferred_normalisation_agrees_with_the_rmsnorm_kernels(cuda_device, mon
   assert err.mean().item() < 1e-2 and (err > 0.1).float().mean().item() < 1e-2
 
 
-_VARIANT_CHILD = r'''
-import json, os, sys
-import torch
-sys.path.insert(0, os.getcwd())
-from music_spectrogram_diffusion_b200 import config, weights
-from tests import helpers as H
-t5 = config.t5_tiny(emb_dim=768, num_heads=12, layers=2, mlp_dim=2048)
-L, B, steps = 256, 8, 8
-params = weights.synthetic_params(t5, L, L, L, seed=6)
-toks, ctx, cmask = H.make_batch(B, L, L, seed=7, pad_second=True)
-dev = torch.device('cuda', 0)
-b = H.torch_batch(toks, ctx, cmask, dev)
-z = torch.randn(B, L, 128, device=dev, generator=torch.Generator(dev).manual_seed(2))
-outs = {}
-for mode in ('0', '1'):
-  os.environ['MSD_FUSED_NORM'] = mode
-  eng = H.build_engine(t5, L, L, L, B, steps, 2.0, params)
-  eng.encode(b['encoder_input_tokens'], b['encoder_continuous_inputs'], b['encoder_continuous_mask'])
-  outs[mode] = [eng.decode_eps(z, 5, c).double().cpu() for c in (True, False)]
-  eng.close()
-rel = [((g - w).abs().mean() / w.abs().mean()).item() for g, w in zip(outs['1'], outs['0'])]
-print('REL ' + json.dumps(rel))
-'''
-
-
-def test_forced_gemm_variant_keeps_the_deferred_normalisation_consistent(cuda_device):
-  """MSD_GEMM_VARIANT=1 (a debugging aid, read once per process) restricts the GEMM tile widths to
-  powers of two.  The deferred normalisation sums one partial row sum per column tile of the
-  residual projection, so the count must follow the tiling that ran: at 4096 rows of d = 768 the
-  forced variant tiles 128 wide (6 partials) where the default picks 192 (4).  Run in a child
-  process with the variant forced: the fused and the stand-alone norm forms must agree as in
-  test_deferred_normalisation_agrees_with_the_rmsnorm_kernels."""
-  import json
-  import os
-  import subprocess
-  import sys
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  env = dict(os.environ, MSD_GEMM_VARIANT='1')
-  r = subprocess.run([sys.executable, '-c', _VARIANT_CHILD], cwd=root, env=env, capture_output=True,
-                     text=True, timeout=900)
-  assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
-  line = [s for s in r.stdout.splitlines() if s.startswith('REL ')][-1]
-  rel = json.loads(line[4:])
-  print(f'MSD_GEMM_VARIANT=1, fused vs stand-alone norm, mean relative difference '
-        f'(conditional, unconditional): {rel}')
-  assert all(x < 1e-2 for x in rel), rel
+def test_deferred_normalisation_agrees_with_the_rmsnorm_kernels_at_base_width(cuda_device, monkeypatch):
+  """The deferred normalisation sums one partial row sum per column tile of the residual
+  projection, so the count must follow the tile width that ran.  At base width (d = 768) and B = 8,
+  on 132 SMs (H100 SXM), the residual projections over 4096 rows run 192 wide (4 partial row sums)
+  and the cross-attention output projection over the 2048 conditional rows 96 wide (8); the
+  t5_small, B = 3 case of test_deferred_normalisation_agrees_with_the_rmsnorm_kernels runs them 64
+  wide (8).  The fused and the stand-alone norm forms must agree as there, for both passes."""
+  t5 = config.t5_tiny(emb_dim=768, num_heads=12, layers=2, mlp_dim=2048)
+  L, B, steps = 256, 8, 8
+  params = weights.synthetic_params(t5, L, L, L, seed=6)
+  toks, ctx, cmask = H.make_batch(B, L, L, seed=7, pad_second=True)
+  b = H.torch_batch(toks, ctx, cmask, cuda_device)
+  z = torch.randn(B, L, 128, device=cuda_device, generator=torch.Generator(cuda_device).manual_seed(2))
+  outs = {}
+  for mode in ('0', '1'):
+    monkeypatch.setenv('MSD_FUSED_NORM', mode)
+    eng = H.build_engine(t5, L, L, L, B, steps, 2.0, params)
+    eng.encode(b['encoder_input_tokens'], b['encoder_continuous_inputs'], b['encoder_continuous_mask'])
+    outs[mode] = [eng.decode_eps(z, 5, c).double().cpu() for c in (True, False)]
+    eng.close()
+  for got, want in zip(outs['1'], outs['0']):
+    rel = ((got - want).abs().mean() / want.abs().mean()).item()
+    assert rel < 1e-2, rel
 
 
 def test_jax_random_stream_on_device_matches_numpy(cuda_device):

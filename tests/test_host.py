@@ -132,7 +132,7 @@ def test_audio_codec_scaling():
     ac.decode(f)
 
 
-def test_c_abi_7_exports_every_declared_symbol(native_lib):
+def test_c_abi_8_exports_every_declared_symbol(native_lib):
   """Every function include/msd_b200.h declares is exported, and nothing is bound twice."""
   hdr = open(os.path.join(ROOT, 'include', 'msd_b200.h')).read()
   hdr = re.sub(r'/\*.*?\*/', '', hdr, flags=re.S)
@@ -142,7 +142,7 @@ def test_c_abi_7_exports_every_declared_symbol(native_lib):
   assert declared == bound, (declared ^ bound)
   for name in declared:
     assert hasattr(native_lib, name), name
-  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 7
+  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 8
   assert isinstance(native_lib.msd_last_error(), bytes)
 
 

@@ -23,27 +23,30 @@ def report(name, got, want, tol):
       print('    bad rows (first 20):', rows[:20].tolist(), ' n=', len(rows))
       print('    bad cols (first 20):', cols[:20].tolist(), ' n=', len(cols))
 
-def probe_gemm(variant=0):
-  print('--- gemm variant', variant)
-  for (M, N, K) in [(128, 64, 64), (256, 128, 64), (256, 192, 128), (256, 256, 256), (128, 256, 768), (1024, 768, 768), (4096, 2304, 768)]:
-    # selection probe: A one-hot -> out[m, n] = W[m % K, n]
-    a = torch.zeros(M, K); a[torch.arange(M), torch.arange(M) % K] = 1.0
-    w = ((torch.arange(K)[:, None] + 2 * torch.arange(N)[None, :]) % 251).float()
-    try:
-      got = engine.op_dense(a.to(dev), w.to(dev), variant).cpu()
-      report(f'gemm-select {M}x{N}x{K}', got, w[torch.arange(M) % K], 0.5)
-    except Exception as e:
-      print('gemm-select', (M, N, K), 'EXC', e)
-      return False
-    g = torch.Generator().manual_seed(0)
-    a = torch.randn(M, K, generator=g).bfloat16().float()
-    w = (torch.randn(K, N, generator=g) / np.sqrt(K)).bfloat16().float()
-    try:
-      got = engine.op_dense(a.to(dev), w.to(dev), variant).cpu()
-      report(f'gemm-rand {M}x{N}x{K}', got, a @ w, 1e-2)
-    except Exception as e:
-      print('gemm-rand', (M, N, K), 'EXC', e)
-      return False
+def probe_gemm():
+  for block_n in (0, 64, 96, 128, 192, 256):
+    print('--- gemm block_n', block_n)
+    for (M, N, K) in [(128, 64, 64), (256, 128, 64), (256, 192, 128), (256, 256, 256), (128, 256, 768), (1024, 768, 768), (4096, 2304, 768)]:
+      if block_n and N % block_n:
+        continue
+      # selection probe: A one-hot -> out[m, n] = W[m % K, n]
+      a = torch.zeros(M, K); a[torch.arange(M), torch.arange(M) % K] = 1.0
+      w = ((torch.arange(K)[:, None] + 2 * torch.arange(N)[None, :]) % 251).float()
+      try:
+        got = engine.op_dense_epilogue(a.to(dev), w.to(dev), 'f32', block_n).cpu()
+        report(f'gemm-select {M}x{N}x{K}', got, w[torch.arange(M) % K], 0.5)
+      except Exception as e:
+        print('gemm-select', (M, N, K), 'EXC', e)
+        return False
+      g = torch.Generator().manual_seed(0)
+      a = torch.randn(M, K, generator=g).bfloat16().float()
+      w = (torch.randn(K, N, generator=g) / np.sqrt(K)).bfloat16().float()
+      try:
+        got = engine.op_dense_epilogue(a.to(dev), w.to(dev), 'f32', block_n).cpu()
+        report(f'gemm-rand {M}x{N}x{K}', got, a @ w, 1e-2)
+      except Exception as e:
+        print('gemm-rand', (M, N, K), 'EXC', e)
+        return False
   return True
 
 def probe_attn():
@@ -87,7 +90,6 @@ def probe_attn():
 if __name__ == '__main__':
   _native.load()
   print(torch.cuda.get_device_name(0))
-  ok = probe_gemm(0)
+  ok = probe_gemm()
   if '--all' in sys.argv:
-    probe_gemm(1)
     probe_attn()

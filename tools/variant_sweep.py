@@ -1,5 +1,5 @@
 """Runs the bench workload once per environment-variable setting (tuning hooks such as
-MSD_ATTN_TAIL / MSD_NORM_VARIANT) in separate processes and prints one summary line each."""
+MSD_ATTN_TAIL / MSD_FUSED_NORM) in separate processes and prints one summary line each."""
 import json, os, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
