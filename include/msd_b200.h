@@ -22,9 +22,9 @@
 extern "C" {
 #endif
 
-/* ABI 8: the plain f32 dense hooks are gone (msd_op_dense_epilogue runs epilogue 1), and block_n
- * alone sets the GEMM tile width (no `variant` in msd_gemm_view_args or msd_bench_gemm). */
-#define MSD_B200_ABI_VERSION 8
+/* ABI 9: msd_op_rmsnorm_view (every launch form of the norm kernel) replaces msd_op_rmsnorm_film,
+ * and msd_op_encoder_inputs runs the encoder's mask and embedding kernels. */
+#define MSD_B200_ABI_VERSION 9
 
 typedef struct msd_ctx msd_ctx;
 
@@ -455,10 +455,61 @@ int msd_op_init_z(const msd_init_z_args* args, void* stream);
 int msd_op_scale_split(const float* feat, void* out_split, int64_t rows, int32_t n_dims, float feat_min,
                        float feat_max, void* stream);
 
-/* LayerNorm (layers.py:632-649) followed by optional FiLM (layers.py:652-666) with explicit
- * scale|bias vector film [2*d] (NULL = none): out f32 (bf16-rounded) [rows, d]. */
-int msd_op_rmsnorm_film(const float* x, const float* gamma, const float* film, int32_t rows,
-                        int32_t d, float* out, void* stream);
+/* One launch of the row-norm kernel on caller-owned device buffers, in any form the engine launches
+ * it: LayerNorm (layers.py:632-649, T5 RMS norm with eps 1e-6), then optionally FiLM (layers.py:
+ * 652-666), to bf16.  Every pointer is a device pointer, 16-byte aligned. */
+typedef struct msd_rmsnorm_view_args {
+  const float* x;             /* f32 [rows, d], contiguous */
+  int32_t rows;
+  int32_t d;                  /* k * 128 <= 1024 */
+  const float* gamma;         /* f32 [d] */
+  void* out;                  /* bf16; output row r' at out + out_off + r' * ldo (r' = r without a
+                                 remap), d values, or [hi | lo | hi] (3 d values) with split3.
+                                 Nothing else is written */
+  int64_t out_off;
+  int32_t ldo;                /* >= d (>= 3 d with split3); with a remap exactly d (3 d) */
+  const float* film;          /* f32 scale | bias rows [2 d] at film + (*step) * film_step_stride +
+                                 film_offset, or NULL (no FiLM) */
+  int64_t film_step_stride;
+  int64_t film_offset;
+  const int32_t* step;        /* device int32 step index, read with film */
+  int32_t split3;             /* 1: write [hi | lo | hi] of the fp32 result (fp32-accurate mode) */
+  int32_t src_len;            /* > 0: remap input row b * src_len + t to output row b * dst_len +
+                                 dst_off + t (the encoders' final norms into the encodings) */
+  int32_t dst_len;
+  int32_t dst_off;
+} msd_rmsnorm_view_args;
+
+/* The norm kernel as *args describes it.  Refused (-1): NULL args or a null pointer, d not k * 128
+ * <= 1024, rows <= 0, ldo below the row written (a remap's ldo other than it), offsets, strides or
+ * ldo not multiples of 4 or negative, FiLM without the step, a remap whose src_len does not divide
+ * rows or whose rows do not fit dst_len, and FiLM together with a remap.  The launch waits for all
+ * earlier work on the stream; synchronises it. */
+int msd_op_rmsnorm_view(const msd_rmsnorm_view_args* args, void* stream);
+
+/* The encoder's front end as msd_encode runs it, on caller-owned device buffers. */
+typedef struct msd_encoder_inputs_args {
+  const int32_t* tokens;      /* int32 [B, T] */
+  const int32_t* ctx_mask;    /* int32 [B, C], or NULL with C == 0 */
+  int32_t B, T, C;            /* T, C multiples of 128; C == 0: no context */
+  int32_t terminal_relative;  /* 1: ctx_seq_len[b] = get_sequence_length(ctx_mask[b]) % C
+                                 (network.py:28-39), 0: zeros; must be 0 with C == 0 */
+  const float* embedding;     /* f32 [vocab, d] */
+  const float* pos;           /* f32 [T, d] */
+  int32_t d;                  /* multiple of 4 */
+  int32_t vocab;
+  uint32_t* bits;             /* [B, (T + C) / 32] key-mask words: bit j of word w of row b is
+                                 tokens[b, 32 w + j] > 0, then ctx_mask[b, 32 (w - T / 32) + j] > 0 */
+  int32_t* ctx_seq_len;       /* [B] */
+  float* x;                   /* f32 [B, T, d] = one_hot(tokens) @ embedding + pos: an id outside
+                                 [0, vocab) embeds as zeros (x = pos) */
+} msd_encoder_inputs_args;
+
+/* The key masks, the context roll and the token encoder's input rows as *args describes them.
+ * Refused (-1): NULL args or a null pointer (ctx_mask only with C > 0), B < 1, T or C not a
+ * multiple of 128, d not a positive multiple of 4, vocab < 1, terminal_relative with C == 0.
+ * Synchronises the stream. */
+int msd_op_encoder_inputs(const msd_encoder_inputs_args* args, void* stream);
 
 /* jax.random.normal of the sampler's stream: step < 0 -> normal(PRNGKey(seed), [n]) (init_z,
  * diffusion_utils.py:462), else normal(fold_in(PRNGKey(seed), step), [n]) (389-390).

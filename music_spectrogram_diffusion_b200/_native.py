@@ -183,6 +183,25 @@ class MsdInitZArgs(ctypes.Structure):
   ]
 
 
+class MsdRmsnormViewArgs(ctypes.Structure):
+  """struct msd_rmsnorm_view_args (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('x', _P), ('rows', _I), ('d', _I), ('gamma', _P), ('out', _P), ('out_off', _L), ('ldo', _I),
+      ('film', _P), ('film_step_stride', _L), ('film_offset', _L), ('step', _P), ('split3', _I),
+      ('src_len', _I), ('dst_len', _I), ('dst_off', _I),
+  ]
+
+
+class MsdEncoderInputsArgs(ctypes.Structure):
+  """struct msd_encoder_inputs_args (include/msd_b200.h)."""
+  __slots__ = ()
+  _fields_ = [
+      ('tokens', _P), ('ctx_mask', _P), ('B', _I), ('T', _I), ('C', _I), ('terminal_relative', _I),
+      ('embedding', _P), ('pos', _P), ('d', _I), ('vocab', _I), ('bits', _P), ('ctx_seq_len', _P), ('x', _P),
+  ]
+
+
 # Every symbol include/msd_b200.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ('msd_last_error', ctypes.c_char_p, []),
@@ -205,7 +224,6 @@ SYMBOLS = [
     ('msd_bench_gemm', ctypes.c_int, [_I, _I, _I, _I, _I, _I, ctypes.POINTER(ctypes.c_float)]),
     ('msd_bench_attention', ctypes.c_int, [_I, _I, _I, _I, _I, ctypes.POINTER(ctypes.c_float)]),
     ('msd_op_attention', ctypes.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
-    ('msd_op_rmsnorm_film', ctypes.c_int, [_P, _P, _P, _I, _I, _P, _P]),
     ('msd_op_jax_normal', ctypes.c_int, [ctypes.c_uint64, _I, ctypes.c_int64, _P, _P]),
     ('msd_op_jax_bits', ctypes.c_int, [ctypes.c_uint64, _I, ctypes.c_int64, _P, _P]),
     ('msd_op_dense_epilogue', ctypes.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _I, _P, _P]),
@@ -220,6 +238,8 @@ SYMBOLS = [
     ('msd_op_init_z', ctypes.c_int, [ctypes.POINTER(MsdInitZArgs), _P]),
     ('msd_op_scale_split', ctypes.c_int,
      [_P, _P, ctypes.c_int64, _I, ctypes.c_float, ctypes.c_float, _P]),
+    ('msd_op_rmsnorm_view', ctypes.c_int, [ctypes.POINTER(MsdRmsnormViewArgs), _P]),
+    ('msd_op_encoder_inputs', ctypes.c_int, [ctypes.POINTER(MsdEncoderInputsArgs), _P]),
     ('msd_op_audio_mel', ctypes.c_int, [_P, _I, ctypes.c_int64, _P, _P, _P, _P]),
     ('msd_op_audio_resample', ctypes.c_int,
      [_P, _I, ctypes.c_int64, _I, _I, _P, _I, _I, _P, _I, _P, ctypes.c_int64, _P]),
@@ -230,7 +250,7 @@ SYMBOLS = [
      [_P, _I, ctypes.c_int64, _P, _P, _P, _P, ctypes.c_float, _I, _P]),
     ('msd_op_griffin_lim_istft', ctypes.c_int, [_P, _P, _I, ctypes.c_int64, _P, _P, _P]),
 ]
-ABI_VERSION = 8  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
+ABI_VERSION = 9  # MSD_B200_ABI_VERSION of include/msd_b200.h this binding was written against
 
 _lib: Optional[ctypes.CDLL] = None
 

@@ -1,7 +1,7 @@
 // Row-wise / element-wise kernels of the DDPM hot path (HBM-bound; vectorised, coalesced):
 //   rmsnorm(+FiLM)   msd/layers.py:632-649 (T5 RMS norm), 652-666 (FiLM x*(1+s)+b)
 //   sampler step     msd/models/diffusion/diffusion_utils.py:398-453, 382-395, 120-163, 215-222
-//   token embedding  msd/layers.py:556-559 + network.py:278-287
+//   token embedding  msd/layers.py:556-559 + network.py:278-287 (one-hot: ids outside the table embed as 0)
 //   feature scaling  msd/audio_codecs.py:166-183
 //   masks            msd/models/diffusion/network.py:28-51, 546; msd/layers.py:341-348
 #include "common.cuh"
@@ -483,10 +483,12 @@ embed_tokens_kernel(const int* tokens, const float* emb, const float* pos, float
   const long long gid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (gid >= static_cast<long long>(rows) * d4) return;
   const int row = static_cast<int>(gid / d4), c = static_cast<int>(gid - static_cast<long long>(row) * d4);
-  int tok = tokens[row];
-  tok = tok < 0 ? 0 : (tok >= vocab ? vocab - 1 : tok);
+  const int tok = tokens[row];
   const int t = row % T;
-  const float4 e = __ldg(reinterpret_cast<const float4*>(emb + static_cast<size_t>(tok) * d) + c);
+  // the reference embeds through one_hot(tok) @ emb (layers.py Embed, one_hot=True): an id outside
+  // [0, vocab) matches no row and embeds as zeros
+  float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (tok >= 0 && tok < vocab) e = __ldg(reinterpret_cast<const float4*>(emb + static_cast<size_t>(tok) * d) + c);
   const float4 pp = __ldg(reinterpret_cast<const float4*>(pos + static_cast<size_t>(t) * d) + c);
   reinterpret_cast<float4*>(x + static_cast<size_t>(row) * d)[c] =
       make_float4(e.x + pp.x, e.y + pp.y, e.z + pp.z, e.w + pp.w);

@@ -688,18 +688,58 @@ int msd_op_scale_split(const float* feat, void* out_split, int64_t rows, int32_t
   return 0;
 }
 
-int msd_op_rmsnorm_film(const float* x, const float* gamma, const float* film, int32_t rows,
-                        int32_t d, float* out, void* stream) {
-  MSD_REQUIRE(x && gamma && out, "msd_op_rmsnorm_film: null argument");
+int msd_op_rmsnorm_view(const msd_rmsnorm_view_args* args, void* stream) {
+  MSD_REQUIRE(args && args->x && args->gamma && args->out, "msd_op_rmsnorm_view: null argument");
+  const msd_rmsnorm_view_args& a = *args;
+  MSD_REQUIRE(a.rows > 0 && a.d > 0 && a.d % 128 == 0 && a.d <= 1024,
+              "msd_op_rmsnorm_view: rows=%d must be > 0 and d=%d k*128 <= 1024", a.rows, a.d);
+  MSD_REQUIRE(a.split3 == 0 || a.split3 == 1, "msd_op_rmsnorm_view: split3 must be 0 or 1");
+  MSD_REQUIRE(a.out_off >= 0 && a.film_offset >= 0 && a.film_step_stride >= 0 && a.src_len >= 0 &&
+                  a.dst_len >= 0 && a.dst_off >= 0,
+              "msd_op_rmsnorm_view: negative offset, stride or length");
+  // the kernel moves 4 values at a time: 16-byte loads of x / gamma / FiLM, 8-byte stores of bf16
+  MSD_REQUIRE(a.out_off % 4 == 0 && a.ldo % 4 == 0 && a.film_offset % 4 == 0 && a.film_step_stride % 4 == 0,
+              "msd_op_rmsnorm_view: out_off, ldo, film_offset and film_step_stride must be multiples of 4");
+  MSD_REQUIRE(((reinterpret_cast<uintptr_t>(a.x) | reinterpret_cast<uintptr_t>(a.gamma) |
+                reinterpret_cast<uintptr_t>(a.film) | reinterpret_cast<uintptr_t>(a.out)) & 15) == 0,
+              "msd_op_rmsnorm_view: x, gamma, film and out must be 16-byte aligned");
+  const int width = a.split3 ? 3 * a.d : a.d;
+  MSD_REQUIRE(a.ldo >= width, "msd_op_rmsnorm_view: ldo=%d below the %d values of a row", a.ldo, width);
+  MSD_REQUIRE(!a.film || a.step, "msd_op_rmsnorm_view: FiLM rows need the device step");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  TempBufs tb;
-  bf16* ob = nullptr;
-  int* zero = nullptr;
-  MSD_TRY(tb.get(&ob, static_cast<size_t>(rows) * d));
-  MSD_TRY(tb.get(&zero, 1));
-  MSD_CUDA_CHECK(cudaMemsetAsync(zero, 0, sizeof(int), st));
-  MSD_TRY(launch_rmsnorm(x, gamma, rows, d, ob, d, film, zero, 0, 0, 0, st));
-  MSD_TRY(launch_bf16_to_f32(ob, out, static_cast<long long>(rows) * d, st));
+  bf16* out = static_cast<bf16*>(a.out) + a.out_off;
+  g_pdl_skip_next = true;   // the inputs were just written by the caller's own kernels
+  if (a.src_len > 0) {
+    MSD_REQUIRE(!a.film, "msd_op_rmsnorm_view: a remapped launch takes no FiLM");
+    MSD_REQUIRE(a.rows % a.src_len == 0 && a.dst_off + a.src_len <= a.dst_len && a.ldo == width,
+                "msd_op_rmsnorm_view: remap of rows=%d in sequences of %d to [%d, +%d) of %d with ldo=%d "
+                "(must be %d)", a.rows, a.src_len, a.dst_off, a.src_len, a.dst_len, a.ldo, width);
+    MSD_TRY(launch_rmsnorm_rows_remap(a.x, a.gamma, a.rows / a.src_len, a.src_len, a.d, out, a.dst_len,
+                                      a.dst_off, st, a.split3));
+  } else {
+    MSD_TRY(launch_rmsnorm(a.x, a.gamma, a.rows, a.d, out, a.ldo, a.film, a.film ? a.step : nullptr,
+                           a.film_step_stride, a.film_offset, a.split3, st));
+  }
+  MSD_CUDA_CHECK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int msd_op_encoder_inputs(const msd_encoder_inputs_args* args, void* stream) {
+  MSD_REQUIRE(args && args->tokens && args->embedding && args->pos && args->bits && args->ctx_seq_len &&
+                  args->x && (args->C == 0 || args->ctx_mask),
+              "msd_op_encoder_inputs: null argument");
+  const msd_encoder_inputs_args& a = *args;
+  MSD_REQUIRE(a.B >= 1 && a.T > 0 && a.T % 128 == 0 && a.C >= 0 && a.C % 128 == 0,
+              "msd_op_encoder_inputs: B=%d must be >= 1, T=%d > 0 and C=%d >= 0 multiples of 128", a.B, a.T,
+              a.C);
+  MSD_REQUIRE(a.d > 0 && a.d % 4 == 0 && a.vocab >= 1, "msd_op_encoder_inputs: d=%d (multiple of 4), vocab=%d",
+              a.d, a.vocab);
+  MSD_REQUIRE(a.terminal_relative == 0 || (a.terminal_relative == 1 && a.C > 0),
+              "msd_op_encoder_inputs: terminal_relative must be 0 or 1, and 0 without a context");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  MSD_TRY(launch_build_masks(a.tokens, a.C > 0 ? a.ctx_mask : nullptr, a.B, a.T, a.C, a.bits, a.ctx_seq_len,
+                             a.terminal_relative, st));
+  MSD_TRY(launch_embed_tokens(a.tokens, a.embedding, a.pos, a.x, a.B, a.T, a.d, a.vocab, st));
   MSD_CUDA_CHECK(cudaStreamSynchronize(st));
   return 0;
 }

@@ -280,12 +280,14 @@ def op_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor,
 
 def op_rmsnorm_film(x: torch.Tensor, gamma: torch.Tensor,
                     film: Optional[torch.Tensor]) -> torch.Tensor:
-  lib = _native.load()
+  """LayerNorm (layers.py:632-649), then FiLM with the scale | bias vector film [2 d] (None = none):
+  f32 (bf16-rounded) [rows, d], through op_rmsnorm_view."""
   rows, d = x.shape
-  out = torch.empty_like(x)
-  _native.check(lib.msd_op_rmsnorm_film(_ptr(x.contiguous()), _ptr(gamma), _ptr(film), rows, d,
-                                        _ptr(out), _stream(x.device)), 'msd_op_rmsnorm_film')
-  return out
+  out = torch.empty(rows, d, dtype=torch.bfloat16, device=x.device)
+  step = None if film is None else torch.zeros(1, dtype=torch.int32, device=x.device)
+  op_rmsnorm_view(x.contiguous(), gamma.contiguous(), out, 0, d,
+                  film=None if film is None else film.contiguous(), step=step)
+  return out.float()
 
 
 EPILOGUES = {'bf16': 0, 'f32': 1, 'resid_f32': 2, 'gated_gelu': 3, 'pos_f32': 4, 'gated_gelu_split3': 5}
@@ -574,6 +576,91 @@ def op_prep_rows(x: torch.Tensor, g: torch.Tensor, g_off: int, g_step_stride: in
   _native.check(_native.load().msd_op_prep_rows(
       _ptr(x), ctypes.c_void_p(g.data_ptr() + 4 * g_off), g_step_stride, _ptr(step), rows, d,
       _ptr(a_out), lda, _ptr(ss_out), _stream(dev)), 'msd_op_prep_rows')
+
+
+def op_rmsnorm_view(x: torch.Tensor, gamma: torch.Tensor, out: torch.Tensor, out_off: int, ldo: int,
+                    film: Optional[torch.Tensor] = None, film_offset: int = 0, film_step_stride: int = 0,
+                    step: Optional[torch.Tensor] = None, split3: bool = False, src_len: int = 0,
+                    dst_len: int = 0, dst_off: int = 0) -> None:
+  """The norm kernel in any form the engine launches it (msd_op_rmsnorm_view): x f32 [rows, d] ->
+  rmsnorm(x) gamma, with FiLM (scale | bias rows [2 d] of film at film_offset + step * film_step_stride)
+  when film is given, written in place to the bf16 out at out_off + r * ldo (split3: [hi | lo | hi]).
+  src_len > 0 remaps row b * src_len + t to b * dst_len + dst_off + t.  Views are checked before the
+  library is called."""
+  dev = x.device
+  _check_dev('x', x, torch.float32, dev)
+  if x.dim() != 2:
+    raise ValueError(f'x: expected [rows, d], got {tuple(x.shape)}')
+  rows, d = x.shape
+  if rows <= 0 or d % 128 or not 0 < d <= 1024:
+    raise ValueError(f'x: {rows} rows of d = {d}: d must be k * 128 <= 1024')
+  _check_view('x', x, 0, d, rows, d, 4)
+  _check_vector('gamma', gamma, 0, d, dev)
+  _check_dev('out', out, torch.bfloat16, dev)
+  width = 3 * d if split3 else d
+  out_rows = rows
+  if src_len:
+    if src_len < 0 or rows % src_len or dst_off < 0 or dst_off + src_len > dst_len:
+      raise ValueError(f'remap of {rows} rows in sequences of {src_len} to rows [{dst_off}, '
+                       f'{dst_off + src_len}) of {dst_len}')
+    if film is not None:
+      raise ValueError('a remapped launch takes no FiLM')
+    if ldo != width:
+      raise ValueError(f'a remapped launch writes rows of {width} values: ldo must be {width}')
+    out_rows = rows // src_len * dst_len
+  _check_view('out', out, out_off, ldo, out_rows, width, 2)
+  if film is not None:
+    if step is None:
+      raise ValueError('FiLM rows need the device step')
+    _check_vector('film', film, film_offset + _step_value(step, dev) * film_step_stride, 2 * d, dev)
+    if film_offset % 4 or film_step_stride % 4 or film_step_stride < 0:
+      raise ValueError(f'film: offset {film_offset} / step stride {film_step_stride} must be '
+                       'non-negative multiples of 4')
+  args = _native.MsdRmsnormViewArgs(
+      x=_ptr(x), rows=rows, d=d, gamma=_ptr(gamma), out=_ptr(out), out_off=out_off, ldo=ldo, film=_ptr(film),
+      film_step_stride=film_step_stride, film_offset=film_offset, step=_ptr(step), split3=int(bool(split3)),
+      src_len=src_len, dst_len=dst_len, dst_off=dst_off)
+  _native.check(_native.load().msd_op_rmsnorm_view(ctypes.byref(args), _stream(dev)), 'msd_op_rmsnorm_view')
+
+
+def op_encoder_inputs(tokens: torch.Tensor, ctx_mask: Optional[torch.Tensor], embedding: torch.Tensor,
+                      pos: torch.Tensor, terminal_relative: bool, bits: torch.Tensor,
+                      ctx_seq_len: torch.Tensor, x: torch.Tensor) -> None:
+  """The encoder's front end as msd_encode runs it (msd_op_encoder_inputs): from tokens int32 [B, T]
+  and ctx_mask int32 [B, C] (None: no context, C = 0), writes the key-mask words bits int32 storage
+  [B, (T + C) / 32], the context roll ctx_seq_len int32 [B] and the token encoder's input rows x f32
+  [B, T, d] = one_hot(tokens) embedding [vocab, d] + pos [T, d].  Buffers are checked before the
+  library is called."""
+  dev = tokens.device
+  _check_dev('tokens', tokens, torch.int32, dev)
+  if tokens.dim() != 2 or not tokens.is_contiguous():
+    raise ValueError(f'tokens: expected a contiguous [B, T], got {tuple(tokens.shape)}')
+  b, t = tokens.shape
+  c = 0
+  if ctx_mask is not None:
+    _check_dev('ctx_mask', ctx_mask, torch.int32, dev)
+    if ctx_mask.dim() != 2 or ctx_mask.shape[0] != b or not ctx_mask.is_contiguous():
+      raise ValueError(f'ctx_mask: expected a contiguous [{b}, C], got {tuple(ctx_mask.shape)}')
+    c = ctx_mask.shape[1]
+  if b < 1 or t <= 0 or t % 128 or c % 128 or (ctx_mask is not None and c == 0):
+    raise ValueError(f'B = {b} must be >= 1, T = {t} and C = {c} positive multiples of 128')
+  if terminal_relative and c == 0:
+    raise ValueError('terminal_relative positions need a context')
+  _check_dev('embedding', embedding, torch.float32, dev)
+  if embedding.dim() != 2 or not embedding.is_contiguous() or embedding.shape[0] < 1:
+    raise ValueError(f'embedding: expected a contiguous [vocab, d], got {tuple(embedding.shape)}')
+  vocab, d = embedding.shape
+  if d % 4:
+    raise ValueError(f'd = {d} must be a multiple of 4')
+  _check_flat('pos', pos, torch.float32, dev, t * d)
+  _check_flat('bits', bits, torch.int32, dev, b * (t + c) // 32)
+  _check_flat('ctx_seq_len', ctx_seq_len, torch.int32, dev, b)
+  _check_flat('x', x, torch.float32, dev, b * t * d)
+  args = _native.MsdEncoderInputsArgs(
+      tokens=_ptr(tokens), ctx_mask=_ptr(ctx_mask), B=b, T=t, C=c, terminal_relative=int(bool(terminal_relative)),
+      embedding=_ptr(embedding), pos=_ptr(pos), d=d, vocab=vocab, bits=_ptr(bits), ctx_seq_len=_ptr(ctx_seq_len),
+      x=_ptr(x))
+  _native.check(_native.load().msd_op_encoder_inputs(ctypes.byref(args), _stream(dev)), 'msd_op_encoder_inputs')
 
 
 STEP_COLS = 16   # floats per diffusion step in the sampler table (msd_get_step_table)

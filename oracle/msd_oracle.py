@@ -189,8 +189,12 @@ def zero_activations_if_masked(y: Tensor, mask: Tensor) -> Tensor:
 
 
 def embed(ids: Tensor, embedding: Tensor) -> Tensor:
-  """msd/layers.py:556-559: the one-hot matmul is a gather in exact arithmetic."""
-  return embedding[ids.long()]
+  """msd/layers.py:556-559 with one_hot=True: one_hot(ids) @ embedding, a gather in exact arithmetic.
+  An id outside [0, vocab) matches no row of the one-hot and embeds as zeros."""
+  ids = ids.long()
+  valid = (ids >= 0) & (ids < embedding.shape[0])
+  rows = embedding[torch.where(valid, ids, torch.zeros_like(ids))]
+  return torch.where(valid.unsqueeze(-1), rows, torch.zeros_like(rows))
 
 
 def sinusoidal_table(max_len: int, features: int, rng: np.random.Generator,

@@ -316,6 +316,100 @@ def test_deferred_normalisation_agrees_with_the_rmsnorm_kernels_at_base_width(cu
     assert rel < 1e-2, rel
 
 
+# ---- t5_large's width (gin/models/diffusion/context/t5_large.gin: d 1024, 16 heads, mlp 2816) --------
+# The widest network validate() accepts: the norm kernel's ITERS 8 instance, 16 partial row sums per
+# row when the residual projections run 64 wide, film_bias with K = 1024, 16 heads and a 5632-wide
+# gated projection.  Two layers, B = 2, lengths 256.
+@pytest.fixture(scope='module')
+def large_width():
+  t5 = config.t5_tiny(emb_dim=1024, num_heads=16, layers=2, mlp_dim=2816)
+  L = 256
+  return t5, L, weights.synthetic_params(t5, L, L, L, seed=8)
+
+
+def _large_width_oracle(t5, L, params, toks, ctx, cmask, steps):
+  oc = H.oracle_config(t5, steps, 2.0)
+  P = O.params_to(params)
+  cb = H.torch_batch(toks, ctx, cmask)
+  encs = O.encode(P, oc, cb['encoder_input_tokens'],
+                  O.scale_features(cb['encoder_continuous_inputs'], oc, clip=True),
+                  cb['encoder_continuous_mask'])
+  return oc, P, encs
+
+
+def test_decode_eps_at_t5_large_width(cuda_device, large_width):
+  """decode_eps against the oracle with test_decode_eps's bound, conditioned and unconditioned."""
+  t5, L, params = large_width
+  B, steps = 2, 16
+  toks, ctx, cmask = H.make_batch(B, L, L, seed=9)
+  eng = H.build_engine(t5, L, L, L, B, steps, 2.0, params)
+  b = H.torch_batch(toks, ctx, cmask, cuda_device)
+  eng.encode(b['encoder_input_tokens'], b['encoder_continuous_inputs'], b['encoder_continuous_mask'])
+  oc, P, encs = _large_width_oracle(t5, L, params, toks, ctx, cmask, steps)
+  z = torch.randn(B, L, 128, generator=torch.Generator().manual_seed(3))
+  for conditioned in (True, False):
+    flag = 1.0 if conditioned else 0.0
+    for step_i in (steps - 1, 5, 0):
+      got = eng.decode_eps(z.to(cuda_device), step_i, conditioned).cpu()
+      t = np.float32(step_i + 1.0) / np.float32(steps)
+      want = O.decode(P, oc, [(e * flag, m * flag) for e, m in encs], z, torch.full((B,), float(t)))
+      rel = ((got - want).abs().max() / want.abs().max()).item()
+      print(f'd=1024 cond={conditioned} step {step_i}: rel max err {rel:.3e}')
+      assert rel < 3e-2, f'cond={conditioned} step {step_i}: rel max err {rel}'
+  eng.close()
+
+
+def test_deferred_normalisation_agrees_with_the_rmsnorm_kernels_at_t5_large_width(cuda_device, monkeypatch,
+                                                                                    large_width):
+  """The fused and the stand-alone norm forms agree as in
+  test_deferred_normalisation_agrees_with_the_rmsnorm_kernels_at_base_width, for both passes."""
+  t5, L, params = large_width
+  B, steps = 2, 8
+  toks, ctx, cmask = H.make_batch(B, L, L, seed=7, pad_second=True)
+  b = H.torch_batch(toks, ctx, cmask, cuda_device)
+  z = torch.randn(B, L, 128, device=cuda_device, generator=torch.Generator(cuda_device).manual_seed(2))
+  outs = {}
+  for mode in ('0', '1'):
+    monkeypatch.setenv('MSD_FUSED_NORM', mode)
+    eng = H.build_engine(t5, L, L, L, B, steps, 2.0, params)
+    eng.encode(b['encoder_input_tokens'], b['encoder_continuous_inputs'], b['encoder_continuous_mask'])
+    outs[mode] = [eng.decode_eps(z, 5, c).double().cpu() for c in (True, False)]
+    eng.close()
+  for got, want in zip(outs['1'], outs['0']):
+    rel = ((got - want).abs().mean() / want.abs().mean()).item()
+    print(f'd=1024 fused vs stand-alone norm: rel mean err {rel:.3e}')
+    assert rel < 1e-2, rel
+
+
+def test_fp32_accurate_decoder_forward_at_t5_large_width(cuda_device, large_width):
+  """precision='fp32_accurate' at d = 1024 within test_fp32_accurate_decoder_forward's bounds: the
+  encodings (split final norms of both encoders) and one decoder forward per pass."""
+  t5, L, params = large_width
+  B, steps = 2, 16
+  toks, ctx, cmask = H.make_batch(B, L, L, seed=9, ctx_masks=[1, 1])
+  cmask[1, 40:] = 0
+  eng = H.build_engine(t5, L, L, L, B, steps, 2.0, params, precision='fp32_accurate')
+  b = H.torch_batch(toks, ctx, cmask, cuda_device)
+  eng.encode(b['encoder_input_tokens'], b['encoder_continuous_inputs'], b['encoder_continuous_mask'])
+  oc, P, encs = _large_width_oracle(t5, L, params, toks, ctx, cmask, steps)
+  want = torch.cat([encs[0][0], encs[1][0]], dim=1)
+  valid = torch.cat([encs[0][1], encs[1][1]], dim=1) > 0
+  err = ((eng.encodings().cpu() - want).abs() * valid.unsqueeze(-1)).max().item()
+  print(f'd=1024 fp32-accurate encodings: max err {err:.3e}')
+  assert err < 2e-3, f'encodings: {err}'
+  z = torch.randn(B, L, 128, generator=torch.Generator().manual_seed(3))
+  for conditioned in (True, False):
+    flag = 1.0 if conditioned else 0.0
+    for step_i in (steps - 1, 5, 0):
+      got = eng.decode_eps(z.to(cuda_device), step_i, conditioned).cpu()
+      t = np.float32(step_i + 1.0) / np.float32(steps)
+      ref = O.decode(P, oc, [(e * flag, m * flag) for e, m in encs], z, torch.full((B,), float(t)))
+      rel = ((got - ref).abs().max() / ref.pow(2).mean().sqrt()).item()
+      print(f'd=1024 fp32-accurate cond={conditioned} step {step_i}: {rel:.3e}')
+      assert rel < 2e-3, f'cond={conditioned} step {step_i}: {rel}'
+  eng.close()
+
+
 def test_jax_random_stream_on_device_matches_numpy(cuda_device):
   """rng_kind = 1: the sampler's noise is jax.random.normal of PRNGKey(seed) / fold_in(key, i)
   (inference.py:203; diffusion_utils.py:389-390, 462).  Device draw vs jax_rng.py (numpy), which

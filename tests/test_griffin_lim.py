@@ -229,6 +229,9 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = 'music_spectrogram_diffusion_b200/csrc'
 # kernels changed on purpose since the shared headers came in: compared as that commit built them
 CHANGED_SINCE = {'sampler_step_kernel'}
+# kernels changed on purpose later, not compared: the token embedding now gives an id outside the table
+# a zero row, as the reference's one-hot embedding does (tests/test_gpu_row_kernels.py checks it bit for bit)
+CHANGED_LATER = {'embed_tokens_kernel'}
 
 
 def _sass(root, src, out_dir):
@@ -276,4 +279,5 @@ def test_shared_headers_leave_encoder_and_sampler_sass_unchanged(tmp_path):
     if changed:
       b.update({k: v for k, v in _sass(at_headers, src, at_headers).items() if k in changed})
     for k in a:
-      assert a[k] == b[k], f'{src}: SASS of {k} differs from the parent commit'
+      if not any(n in k for n in CHANGED_LATER):
+        assert a[k] == b[k], f'{src}: SASS of {k} differs from the parent commit'

@@ -132,7 +132,7 @@ def test_audio_codec_scaling():
     ac.decode(f)
 
 
-def test_c_abi_8_exports_every_declared_symbol(native_lib):
+def test_c_abi_9_exports_every_declared_symbol(native_lib):
   """Every function include/msd_b200.h declares is exported, and nothing is bound twice."""
   hdr = open(os.path.join(ROOT, 'include', 'msd_b200.h')).read()
   hdr = re.sub(r'/\*.*?\*/', '', hdr, flags=re.S)
@@ -142,7 +142,7 @@ def test_c_abi_8_exports_every_declared_symbol(native_lib):
   assert declared == bound, (declared ^ bound)
   for name in declared:
     assert hasattr(native_lib, name), name
-  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 8
+  assert native_lib.msd_abi_version() == _native.ABI_VERSION == 9
   assert isinstance(native_lib.msd_last_error(), bytes)
 
 
@@ -260,7 +260,8 @@ C_STRUCTS = {
     _native.MsdAttentionViewArgs: 'msd_attention_view_args', _native.MsdGemmPrep: 'msd_gemm_prep',
     _native.MsdGemmRowScale: 'msd_gemm_row_scale', _native.MsdGemmViewArgs: 'msd_gemm_view_args',
     _native.MsdNoiseStreams: 'msd_noise_streams', _native.MsdSamplerStepArgs: 'msd_sampler_step_args',
-    _native.MsdInitZArgs: 'msd_init_z_args',
+    _native.MsdInitZArgs: 'msd_init_z_args', _native.MsdRmsnormViewArgs: 'msd_rmsnorm_view_args',
+    _native.MsdEncoderInputsArgs: 'msd_encoder_inputs_args',
 }
 
 
@@ -285,10 +286,12 @@ def _header_field_names(hdr: str, cname: str):
   return names
 
 
-def test_ctypes_structs_match_header(tmp_path):
-  """Every ctypes struct of the binding declares the members of its C struct in the same order, and
-  a C compiler gives the struct, and every member (nested ones too), the size and offset ctypes
-  gives it: a field missing, reordered or resized on either side fails here, without a GPU."""
+def test_ctypes_and_header_structs_match(tmp_path):
+  """The binding and include/msd_b200.h describe the same structs: every ctypes struct of the binding
+  mirrors a C struct, every C struct with a body has a ctypes twin, each declares the same members in
+  the same order, and a C compiler gives the struct, and every member (nested ones too), the size and
+  offset ctypes gives it: a struct or field missing, reordered or resized on either side fails here,
+  without a GPU."""
   import shutil
   import subprocess
   if not shutil.which('gcc'):
@@ -296,6 +299,7 @@ def test_ctypes_structs_match_header(tmp_path):
   defined = {v for v in vars(_native).values() if isinstance(v, type) and issubclass(v, ctypes.Structure)}
   assert defined == set(C_STRUCTS)
   hdr = re.sub(r'/\*.*?\*/', '', open(os.path.join(ROOT, 'include', 'msd_b200.h')).read(), flags=re.S)
+  assert set(re.findall(r'typedef struct (\w+) \{', hdr)) == set(C_STRUCTS.values())
   prints, want = [], []
   for cls, cname in C_STRUCTS.items():
     assert _header_field_names(hdr, cname) == [name for name, _ in cls._fields_], cname

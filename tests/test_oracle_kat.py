@@ -197,3 +197,22 @@ def test_model_output_conversions_are_consistent():
   np.testing.assert_allclose(ec, eps, rtol=1e-9)
   with pytest.raises(ValueError, match='Unknown model_output'):
     O.x0_and_eps_from_model_output(z, eps, ls, 'x0_and_eps')
+
+
+def test_embed_is_the_one_hot_product():
+  """layers.py Embed with one_hot=True (network.py:278-284): one_hot(ids) @ embedding with the
+  one-hot built as ids[..., None] == iota, so an id >= vocab or < 0 matches no row and embeds as
+  zeros (not a clamped or wrapped row)."""
+  vocab, d = 11, 6
+  g = torch.Generator().manual_seed(0)
+  emb = torch.randn(vocab, d, dtype=torch.float64, generator=g)
+  ids = torch.tensor([[0, 1, vocab - 1, vocab, vocab + 5, 2 ** 31 - 1, -1, -vocab],
+                      [5, -2 ** 31, 3, vocab - 1, 0, vocab, 7, 2]], dtype=torch.int32)
+  one_hot = (ids.long().unsqueeze(-1) == torch.arange(vocab)).double()
+  want = one_hot @ emb
+  got = O.embed(ids, emb)
+  assert got.shape == want.shape and got.dtype == torch.float64
+  assert torch.equal(got, want)
+  outside = (ids < 0) | (ids >= vocab)
+  assert outside.sum() == 7 and bool((got[outside] == 0).all())
+  assert torch.equal(got[~outside], emb[ids[~outside].long()])
